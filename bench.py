@@ -37,7 +37,7 @@ METRIC = "env_steps_per_sec"
 UNIT = "env-steps/s"
 
 # The headline (default) workload is BASELINE.json configs[2]; the other two configs that fit one GPU are selectable
-# with --workload for the per-config numbers recorded in profiles/ (they are not the bench line the driver reads).
+# with --workload (they are not the bench line the driver reads).
 WORKLOADS = {
     "quadruped_xpbd": dict(
         config="BASELINE.json configs[2]", scene="quadruped", solver="xpbd", envs=4096, substeps=4, fps=50, kernel="xpbd_step_kernel",
@@ -105,7 +105,11 @@ def parse_args():
                    help="CollisionPipeline(export_contacts=False): the solver reads the contact blocks, the reference-layout Contacts arrays "
                         "are not written (an RL loop that never looks at them); NOT the default, the headline keeps the export")
     p.add_argument("--gather", default="peer", choices=["peer", "nccl"], help="N > 1: end-of-frame state gather mechanism")
+    p.add_argument("--dump-outputs", metavar="DIR", default=None,
+                   help="after the timed steps, write what the last timed step computed (rank 0's shard) as DIR/<name>.npy")
     a = p.parse_args()
+    if a.dump_outputs and a.impl != "native":
+        p.error("--dump-outputs writes the native arm's outputs; it does not apply to --impl reference")
     select_workload(a.workload)
     if a.envs is None:
         a.envs = WL["envs"]
@@ -290,13 +294,13 @@ def run_native(args):
     def timed(fn, steps, warmup, sampler=None):
         if sampler:
             sampler.start()  # before the warm-up and the barrier: forking nvidia-smi costs rank 0 several ms - inside the synchronised
-            #                  region that start-up skew is what every other rank then waits for in the final drain (N = 4: 5 ms / 50 frames)
+            #                  region that start-up skew is what every other rank then waits for in the final drain
         for _ in range(warmup):
             fn()
         barrier()
         ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(steps)]
         for a, b in ev:
-            flush.zero_()  # evict L2 (126 MB) between timed steps; not inside the timed events
+            flush.zero_()  # evict L2 (50 MB on an H100) between timed steps; not inside the timed events
             a.record()
             fn()
             b.record()
@@ -319,6 +323,8 @@ def run_native(args):
 
     sampler = ClockSampler(local_rank) if rank == 0 else None
     total_ms, clocks = timed(step_device, args.steps, max(args.warmup, 3), sampler)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, state_0, contacts if not args.no_export_contacts else None)
     env_steps = envs * world * SUBSTEPS * args.steps
     value = env_steps / (total_ms * 1e-3)
     frame_ms = np.asarray(timed.last_per_step)  # rank-local per-frame device times (SURVEY.md §8(d) extras)
@@ -406,8 +412,8 @@ def run_native(args):
         pipeline.collide(state_0, contacts)
         solver.step(state_0, state_1, control, contacts, DT)
     for _ in range(reps):
-        # same cache state as inside a frame (collide has just written the contact blocks): the kernel's share of the frame
-        # then matches the ncu launch list (profiles/*launch_list*); the frame-level timing above is the L2-flushed one
+        # same cache state as inside a frame (collide has just written the contact blocks); the frame-level timing above is
+        # the L2-flushed one
         pipeline.collide(state_0, contacts)
         a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         a.record()
@@ -426,18 +432,9 @@ def run_native(args):
             peaks = json.load(f)
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    # measured DRAM traffic of ONE launch of the dominant kernel: dram__bytes_read.sum + dram__bytes_write.sum of the committed
-    # `ncu --set full` capture for this workload (profiles/traffic.json names the report it was read from); null when no capture
-    # of the current kernel at this size is committed
+    peak = float(peaks.get("hbm_gbs", 3350.0))  # fallback: the H100 SXM data sheet's HBM3 bandwidth, not a measured rate
+    # measured DRAM traffic of one launch of the dominant kernel: no hardware-counter capture of this build is recorded
     traffic = traffic_src = None
-    try:
-        with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-            t = json.load(f).get(f"{args.workload}:{envs}")
-        if t:
-            traffic, traffic_src = float(t["dram_bytes"]), t["source"]
-    except Exception:
-        pass
     no_model = (alg_bytes_env - WL["model_bytes"]) * envs / (kern_ms * 1e-3) / 1e9
     roofline = {
         "bound": "hbm", "kernel": WL["kernel"], "achieved": achieved, "peak": peak, "unit": "GB/s",
@@ -483,6 +480,37 @@ def run_native(args):
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()
+
+
+DUMP_BYTES = 64 * 1024 * 1024
+
+
+def dump_outputs(out_dir, state, contacts):
+    """--dump-outputs: the arrays a caller of the timed frame receives - the advanced state (body pose / twist, plus the joint
+    coordinates Featherstone writes) and the exported contacts of the last substep - as float32 (float64 for integer arrays) .npy
+    files.  Above DUMP_BYTES in all, every array keeps the same fixed, seeded sample of its rows (indices in <name>_rows.npy)."""
+    torch.cuda.synchronize()
+    arrays = {"body_q": state.body_q, "body_qd": state.body_qd}
+    if WL["solver"] == "featherstone":
+        arrays.update(joint_q=state.joint_q, joint_qd=state.joint_qd)
+    if contacts is not None:
+        n = int(contacts.rigid_contact_count.item())
+        arrays["rigid_contact_count"] = contacts.rigid_contact_count
+        for name in ("shape0", "shape1", "point0", "point1", "offset0", "offset1", "normal", "margin0", "margin1"):
+            arrays["rigid_contact_" + name] = getattr(contacts, "rigid_contact_" + name)[:n]
+    out = {}
+    for name, t in arrays.items():
+        a = t.detach().cpu().numpy()
+        out[name] = a.astype(np.float32) if a.dtype.kind == "f" else a.astype(np.float64)
+    total = sum(a.nbytes for a in out.values())
+    frac = 1.0 if total <= DUMP_BYTES else 0.99 * DUMP_BYTES / sum(a.nbytes + 8 * a.shape[0] for a in out.values())
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in out.items():
+        if frac < 1.0 and a.shape[0] > 1:
+            rows = np.sort(np.random.default_rng(0).choice(a.shape[0], max(1, int(a.shape[0] * frac)), replace=False))
+            a = a[rows]
+            np.save(os.path.join(out_dir, name + "_rows.npy"), rows.astype(np.float64))
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def fast_twin_measurement(args, envs):

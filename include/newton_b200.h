@@ -1,5 +1,5 @@
 /*
- * newton_b200.h - C-ABI of the B200-native batched rigid-body stepper.
+ * newton_b200.h - C-ABI of the H100-native batched rigid-body stepper.
  *
  * This is the drop-in boundary (SURVEY.md §8(b)): plain pointers and sizes, no torch / warp
  * types.  Every array uses the reference's element layout so the pointers of a reference

@@ -1,4 +1,4 @@
-"""newton_b200 - B200-native batched rigid-body stepper behind Newton's solver API."""
+"""newton_b200 - H100-native batched rigid-body stepper behind Newton's solver API."""
 from .sim import (  # noqa: F401
     MAXVAL, BodyFlags, Contacts, Control, GeoType, JointDofConfig, JointType, Model, ModelBuilder,
     ModelFlags, ShapeConfig, ShapeFlags, State, StateFlags, eval_fk, eval_ik,

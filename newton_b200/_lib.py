@@ -14,7 +14,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # Floating-point mode of the kernels.  "strict" (default): no FMA contraction, correctly rounded inverse trig - the build that
 # reproduces the CPU oracle bit for bit.  NB2_FP=fast selects the twin library compiled with nvcc's default contraction: same
 # sources, same contact indices / counts on the test scenes, body state within the north-star tolerance (1e-5 relative after 100
-# substeps, tests/test_gpu_fast_fp.py), about 10 % faster on the XPBD step (profiles/r2o_fp_modes.txt).  NB2_LIB overrides both.
+# substeps, tests/test_gpu_fast_fp.py).  NB2_LIB overrides both.
 FP_MODE = os.environ.get("NB2_FP", "strict").lower()
 if FP_MODE not in ("strict", "fast"):
     raise ValueError(f"NB2_FP={FP_MODE!r}: expected 'strict' or 'fast'")
@@ -43,7 +43,7 @@ def lib():
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise Nb2Error(
-                f"{LIB_PATH} is missing - build it with `python -m newton_b200.build` (nvcc, sm_100a). "
+                f"{LIB_PATH} is missing - build it with `python -m newton_b200.build` (nvcc, sm_90a). "
                 "newton_b200 has no CPU or PyTorch fallback for the hot path."
             )
         L = C.CDLL(LIB_PATH)

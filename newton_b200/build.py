@@ -1,4 +1,4 @@
-"""Builds ``libnewton_b200.so`` in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Builds ``libnewton_b200.so`` in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU)."""
 
 from __future__ import annotations
 
@@ -10,14 +10,13 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libnewton_b200.so")
 # The PRODUCT library is built strict-fp: no FMA contraction + correctly rounded trig, so the kernels reproduce the
-# CPU oracle bit for bit (tests/test_gpu_xpbd_parity.py).  Measured cost on B200 (round 2o): 10 % on the XPBD step kernel
-# (137.7 vs 123.7 us, profiles/r2o_fp_modes.txt).  The contracted "fast" twin is selectable with NB2_FP=fast and held to the
+# CPU oracle bit for bit (tests/test_gpu_xpbd_parity.py).  The contracted "fast" twin is selectable with NB2_FP=fast and held to the
 # north-star tolerance instead of bit equality (tests/test_gpu_fast_fp.py).
 LIB_FAST = os.path.join(HERE, "libnewton_b200_fast.so")
 STRICT_FLAGS = ["-fmad=false", "-DNB2_STRICT_FP=1"]
 SOURCES = ["nb2_api.cu", "nb2_collide.cu", "nb2_xpbd.cu", "nb2_featherstone.cu", "nb2_selection.cu", "nb2_peer.cu", "nb2_match.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "--expt-relaxed-constexpr",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--expt-relaxed-constexpr",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-O2",
 ]
 

@@ -397,8 +397,8 @@ static nb2_status build_tables(nb2_model* m, const nb2_model_desc& d) {
     m->lanes_per_env =
         std::min(32, std::max(8, pow2_at_least(std::max({dv.max_env_bodies, dv.max_env_joints, std::min(dv.max_env_pairs, 32)}))));
     {   // small batches cannot fill the GPU with warps: give each environment a full warp so its contact / pair loops need
-        // fewer rounds (measured on 512 box stacks: xpbd_step 90 -> 68 us); large batches keep the narrowest group that fits
-        int sms = 148;
+        // fewer rounds; large batches keep the narrowest group that fits
+        int sms = 132;
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, m->device);
         while (m->lanes_per_env < 32 && (long long)E * m->lanes_per_env / 32 < 4LL * sms) m->lanes_per_env *= 2;
     }
@@ -846,6 +846,6 @@ nb2_status nb2_eval_ik(nb2_model* model, const float* body_q, const float* body_
 
 const char* nb2_last_error(void) { return g_last_error.c_str(); }
 int64_t nb2_kernel_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
-const char* nb2_version(void) { return "newton_b200 0.1 (sm_100a)"; }
+const char* nb2_version(void) { return "newton_b200 0.1 (sm_90a)"; }
 
 }  // extern "C"

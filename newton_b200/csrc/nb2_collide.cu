@@ -1,7 +1,7 @@
-// nb2_collide.cu - fused per-environment collision pipeline for sm_100a.
+// nb2_collide.cu - fused per-environment collision pipeline for sm_90a.
 //
 // One sub-warp group of L lanes owns one environment (a CTA is a single warp holding 32/L environments, so every
-// synchronisation is a __syncwarp and ~14 independent CTAs per SM cover 4096 environments on 148 SMs in one wave):
+// synchronisation is a __syncwarp and ~16 independent CTAs per SM cover 4096 environments on 132 SMs in one wave):
 //
 //   phase 1  shape world transforms + AABBs          (reference sim/collide.py:283-472 compute_shape_aabbs)
 //   phase 2  explicit-pair AABB test                 (reference geometry/broad_phase_nxn.py:29-69)
@@ -393,7 +393,7 @@ NB2_DEV ShapeMotion ld_motion(const SlotMotionRec& r) {
 // CONVEX = false is instantiated for models none of whose pairs can reach the generic convex path (decided per pair type at
 // nb2_model_create): the analytic-only kernel carries neither the MPR / GJK / manifold code nor its registers and stack.
 // WARPS warps per CTA (each warp = 32/L environments): the kernel is a straight line every warp walks once, so one-warp CTAs each
-// fetch the whole instruction stream cold (48 % `stall_no_inst`, profiles/r1f_collide_kernel_quadruped.txt); warps of one CTA
+// fetch the whole instruction stream cold (`stall_no_inst`); warps of one CTA
 // start together and share the fetches.
 // EXPORT = true also writes the reference-layout `Contacts` arrays in the same launch (the separate contact_export_kernel is gone from
 // the default path): a CTA ("tile") knows its environments' contact counts after the pair loop; the offset of its first contact in the
@@ -1133,8 +1133,8 @@ __global__ void __launch_bounds__(1024) contact_scan_kernel(const int* __restric
 
 // SELF_SCAN (batches up to 8192 environments): one pass - every CTA (4 environments, one warp each) first sums the contact
 // counts of all environments before its own (E/128 coalesced int loads per thread out of L2; exact integer arithmetic, so
-// the offsets equal the scan's) and then scatters its environments' contact blocks; this saves the single-CTA scan launch
-// (6 us of a 40 us collide stage at 4096 envs).  The sum is O(E^2 / 128) over the grid, so larger batches keep the
+// the offsets equal the scan's) and then scatters its environments' contact blocks; this saves the single-CTA scan
+// launch.  The sum is O(E^2 / 128) over the grid, so larger batches keep the
 // separate contact_scan_kernel and read its offsets.
 template <bool SELF_SCAN>
 __global__ void __launch_bounds__(128) contact_export_kernel(DevModel M, nb2_contacts_view out) {
@@ -1424,7 +1424,7 @@ static nb2_status launch_collide_L(nb2_model* m, const float* body_q, const nb2_
     static const int forced = std::getenv("NB2_COLLIDE_WARPS") ? std::atoi(std::getenv("NB2_COLLIDE_WARPS")) : 0;
     int warps = forced;
     if (warps <= 0) {  // as many warps per CTA as the batch puts on every SM, up to 8
-        int sms = 148;
+        int sms = 132;
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, m->device);
         const long long total_warps = (M.env_count + (32 / L) - 1) / (32 / L);
         warps = (total_warps + sms - 1) / sms >= 8 ? 8 : 1;
@@ -1475,11 +1475,10 @@ nb2_status launch_collide(nb2_model* m, const float* body_q, const nb2_contacts_
     }
     if (M.dyn_pairs && (st = launch_broadphase(m, body_q, s)) != NB2_OK) return st;
     // NB2_COLLIDE_FUSED_EXPORT=1: the `Contacts` arrays are written by the collide kernel itself (EXPORT = true, tile chain with
-    // decoupled look-back).  Measured on B200 it LOSES to the two-kernel path (collide, then contact_export_kernel): 4096 quadruped
-    // envs, frame 690.1 vs 678.3 us L2-warm, 733.8 vs 718.0 us with L2 flushed (profiles/r2j_fused_export_ab.txt) - the 256 tiles of
-    // a single-wave launch all reach the look-back at the same time and serialise on it.  So the default is the two-kernel path.
+    // decoupled look-back).  The tiles of a single-wave launch all reach the look-back at the same time and serialise on it, so the
+    // default is the two-kernel path (collide, then contact_export_kernel).
     static const bool fused = std::getenv("NB2_COLLIDE_FUSED_EXPORT") && std::atoi(std::getenv("NB2_COLLIDE_FUSED_EXPORT")) != 0;
-    // one lane per contact in the write-out (NB2_COLLIDE_LANE_PER_CONTACT=0: one lane per pair, the round-1 arrangement; A/B in profiles/)
+    // one lane per contact in the write-out (NB2_COLLIDE_LANE_PER_CONTACT=0: one lane per pair, the round-1 arrangement)
     static const bool lane_per_contact = !(std::getenv("NB2_COLLIDE_LANE_PER_CONTACT") && std::atoi(std::getenv("NB2_COLLIDE_LANE_PER_CONTACT")) == 0);
     m->dev.lane_per_contact = lane_per_contact ? 1 : 0;
     // speculative contacts live in the generic (CONVEX = true) instantiation only, with the two-kernel export

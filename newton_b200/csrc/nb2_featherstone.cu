@@ -1,4 +1,4 @@
-// nb2_featherstone.cu - fused articulated-body step for sm_100a (reference SolverFeatherstone.step,
+// nb2_featherstone.cu - fused articulated-body step for sm_90a (reference SolverFeatherstone.step,
 // solvers/featherstone/solver_featherstone.py:461-1066; kernels in solvers/featherstone/kernels.py).
 //
 // The reference spends ~16 launches per substep, walks every articulation with ONE thread (FK, RNEA forward /
@@ -252,7 +252,7 @@ NB2_DEV Xf joint_transform(const nb2_model_desc& d, int type, int axis_start, in
 struct FsSmem {
     float *bq, *bqc, *vs, *as, *fb, *ft, *fe, *qdfk, *Is, *so, *fs, *S, *qd_in, *jf, *tau, *qdd, *qd_out, *H, *jq, *P;
     // joint headers staged once per substep: the level passes index these instead of going to global memory for every joint's
-    // type / parent / child / depth / offsets in every pass (25 % of the stall samples were those L1 round trips)
+    // type / parent / child / depth / offsets in every pass (L1 round trips that stalled the level passes)
     int *h_type, *h_parent, *h_child, *h_depth, *h_dim, *h_q, *h_qd;
 };
 NB2_DEV size_t fs_smem_floats(const DevModel& M) {
@@ -393,12 +393,13 @@ __device__ __noinline__ void tile_mass_matrix(const float* S, const float* Is, c
 //
 // WARPS warps per CTA, each warp = 32/L environments, with CTA barriers at the phase boundaries (NB2_PHASE): not needed for
 // correctness - a sub-warp group owns its environment - they keep the CTA's warps on the same stretch of this ~9 000-instruction
-// kernel, so the instruction stream is fetched once per CTA instead of once per warp (measured on xpbd_step_kernel:
-// profiles/r2b_xpbd_ab.txt).
+// kernel, so the instruction stream is fetched once per CTA instead of once per warp (the same arrangement as xpbd_step_kernel).
 #define NB2_PHASE()                       \
     do {                                  \
         if (WARPS > 1 && (kflags & 1)) __syncthreads(); \
     } while (0)
+// Residency hint: 14 warps per SM is the most a quadruped's scratch (15.7 KB per two-env warp) leaves room for in 227 KB, so
+// asking for more resident CTAs would only cap the registers (W = 4: 3 CTAs per SM, as shared memory allows).
 template <int L, bool PF, int WARPS, bool TILE>
 __global__ void __launch_bounds__(32 * WARPS, (WARPS >= 14 ? 1 : 14 / WARPS))
 featherstone_step_kernel(DevModel M, nb2_featherstone_params P, nb2_state_view sin, nb2_state_view sout, nb2_control_view ctl, int use_contacts,
@@ -866,7 +867,7 @@ featherstone_step_kernel(DevModel M, nb2_featherstone_params P, nb2_state_view s
             const signed char* dofj = M.dof_joint + ad0;
             const float* Sart = sm.S + 6 * (ad0 - d0);
             // The schedule tables are per articulation, i.e. every environment reads its own copy: inside the batch loop each
-            // lookup was a dependent global load (7 % of the stall samples, profiles/r2o_featherstone_step_kernel_hot_lines.txt).
+            // lookup was a dependent global load.
             // They are staged once - row masks, then the two byte tables - in the dead v_s / a_s block when they fit.
             const int words_body = (nbatch * anj + 3) >> 2, words_row = (nbatch * n + 3) >> 2;
             const bool staged = 2 * n + words_body + words_row <= 12 * M.max_env_bodies;
@@ -1194,8 +1195,8 @@ static nb2_status launch_fs_W(nb2_model* m, const nb2_featherstone_params& p, co
     NB2_CUDA_CHECK(cudaFuncSetAttribute(featherstone_step_kernel<L, PF, WARPS, TILE>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     static const int phase_sync = std::getenv("NB2_FS_PHASE_SYNC") ? std::atoi(std::getenv("NB2_FS_PHASE_SYNC")) : 1;
     // NB2_FS_SHFL_SUBST=1: substitutions with shuffle broadcasts and the products of the backward pass in the upper triangle.  Bit-exact
-    // (the round-2q GPU suite ran with it) but it LOSES: 82.4 vs 80.3 us at 4096 quadruped envs (profiles/r2q_featherstone_subst_ab.txt) -
-    // the divergent per-lane row loops around every shuffle cost more than the barriers they replace.  Default: the round-2p path.
+    // (the GPU suite passes with it), but the divergent per-lane row loops around every shuffle can cost more than the barriers they
+    // replace.  Default: the barrier path.
     static const int shfl_subst = std::getenv("NB2_FS_SHFL_SUBST") ? std::atoi(std::getenv("NB2_FS_SHFL_SUBST")) : 0;
     const int kflags = (phase_sync ? 1 : 0) | (shfl_subst ? 2 : 0);
     static const int min_grid = std::getenv("NB2_FS_MIN_GRID") ? std::atoi(std::getenv("NB2_FS_MIN_GRID")) : 0;  // A/B: idle padding CTAs
@@ -1218,14 +1219,14 @@ static nb2_status launch_fs_LP(nb2_model* m, const nb2_featherstone_params& p, c
     static const int forced = std::getenv("NB2_FS_WARPS") ? std::atoi(std::getenv("NB2_FS_WARPS")) : 0;
     int warps = forced;
     if (warps <= 0) {
-        int sms = 148;
+        int sms = 132;
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, m->device);
         const long long total_warps = (M.env_count + (32 / L) - 1) / (32 / L);
         const long long per_sm = (total_warps + sms - 1) / sms;
-        warps = per_sm <= 1 ? 1 : (per_sm <= 4 ? 4 : 14);
+        warps = per_sm <= 1 ? 1 : (per_sm <= 4 ? 4 : 16);
     }
-    if (warps >= 14 && per_env * 14 > 220 * 1024) warps = 4;
-    if (warps >= 4 && warps < 14 && per_env * 4 > 220 * 1024) warps = 1;
+    if (warps >= 16 && per_env * 16 > 220 * 1024) warps = 4;
+    if (warps >= 4 && warps < 16 && per_env * 4 > 220 * 1024) warps = 1;
     if (p.use_tile_gemm) {
         // the tensor-core variant is compiled for the plain step of the 16- and 32-lane layouts (what use_tile_gemm targets upstream:
         // one 18-dof articulation per world); anything else is refused instead of silently taking the FP32 path
@@ -1234,7 +1235,7 @@ static nb2_status launch_fs_LP(nb2_model* m, const nb2_featherstone_params& p, c
                 set_error("nb2_featherstone_step: use_tile_gemm needs articulations of at most 24 dofs (and >= 12 bodies of scratch per env)");
                 return NB2_ERR_UNSUPPORTED;
             }
-            if (warps >= 14) return launch_fs_W<L, PF, 14, true>(m, p, in, out, ctl, use_contacts, update_mass, dt, s);
+            if (warps >= 16) return launch_fs_W<L, PF, 16, true>(m, p, in, out, ctl, use_contacts, update_mass, dt, s);
             if (warps >= 4) return launch_fs_W<L, PF, 4, true>(m, p, in, out, ctl, use_contacts, update_mass, dt, s);
             return launch_fs_W<L, PF, 1, true>(m, p, in, out, ctl, use_contacts, update_mass, dt, s);
         } else {
@@ -1242,7 +1243,7 @@ static nb2_status launch_fs_LP(nb2_model* m, const nb2_featherstone_params& p, c
             return NB2_ERR_UNSUPPORTED;
         }
     }
-    if (warps >= 14) return launch_fs_W<L, PF, 14, false>(m, p, in, out, ctl, use_contacts, update_mass, dt, s);
+    if (warps >= 16) return launch_fs_W<L, PF, 16, false>(m, p, in, out, ctl, use_contacts, update_mass, dt, s);
     if (warps >= 4) return launch_fs_W<L, PF, 4, false>(m, p, in, out, ctl, use_contacts, update_mass, dt, s);
     return launch_fs_W<L, PF, 1, false>(m, p, in, out, ctl, use_contacts, update_mass, dt, s);
 }

@@ -1,4 +1,4 @@
-// nb2_math.cuh - fp32 vector / quaternion / rigid-transform algebra for the sm_100a kernels.
+// nb2_math.cuh - fp32 vector / quaternion / rigid-transform algebra for the sm_90a kernels.
 //
 // The operation order inside each helper follows NVIDIA Warp's built-ins (the arithmetic the reference
 // kernels are written against: wp.quat_rotate, wp.transform_point, wp.normalize ...; SURVEY.md §8(c)), so

@@ -1,8 +1,8 @@
 // nb2_peer.cu - end-of-frame state gather across the GPUs of one node WITHOUT compute kernels (SURVEY.md §8(e)).
 //
 // The reference design is an ncclAllGather of body_q / body_qd after every frame.  NCCL's all-gather runs as kernels: on a GPU
-// whose solver kernel needs every SM to stay a single wave (13.8 one-warp CTAs per SM at 4096 envs) those kernels push the tail
-// of the wave out (round 1: 90 % weak scaling at N = 8, DESIGN.md §6).  Here every rank owns a symmetric receive buffer
+// whose solver kernel needs every SM to stay a single wave (16 warps per SM at 4096 envs on 132 SMs) those kernels push the tail
+// of the wave out (DESIGN.md §6).  Here every rank owns a symmetric receive buffer
 // (cudaMalloc + CUDA IPC, mapped by all peers); after a frame a rank WRITES its slice into every peer's buffer with the copy
 // engines (cudaMemcpyAsync on peer-mapped pointers: NVLink DMA, no SM), then publishes the frame's sequence number in the
 // peer's flag word; a consumer waits on its own flag words with a stream memory operation (cuStreamWaitValue32: no SM either).

@@ -50,7 +50,7 @@ static bool layout_ok(const nb2_view_layout* L) {
 }
 
 static int copy_grid(long long n) {
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const long long blocks = (n + 255) / 256;

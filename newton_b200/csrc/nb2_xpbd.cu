@@ -1,4 +1,4 @@
-// nb2_xpbd.cu - fused XPBD rigid-body substep for sm_100a (reference SolverXPBD.step, solver_xpbd.py:329-862).
+// nb2_xpbd.cu - fused XPBD rigid-body substep for sm_90a (reference SolverXPBD.step, solver_xpbd.py:329-862).
 //
 // The reference runs `2 + iterations*6 + 1` kernel launches per substep, each re-reading body state from
 // HBM/L2 and summing per-body corrections with float atomics.  Here ONE launch does the whole substep for
@@ -35,12 +35,10 @@ enum { XF_JOINT_CACHE = 1, XF_TMA = 2, XF_PHASE_SYNC = 4, XF_PHASE_SYNC_FINE = 8
 // coefficients and the friction anchors point + offset (odd stride: lanes = consecutive contacts)
 enum { CC_P0 = 0, CC_P1 = 3, CC_N = 6, CC_MSUM = 9, CC_MU = 10, CC_MUT = 11, CC_MUR = 12, CC_Q0 = 13, CC_Q1 = 16, CC_SIZE = 19 };
 
-// Code-size control.  The first kernel version inlined and unrolled everything: 9 400 SASS instructions (150 KB) and
-// 19 % of the stall samples on instruction fetch (profiles/r1a_xpbd_step_kernel.txt).  With one-warp CTAs (round 1) rolled vs.
-// unrolled 3-row joint loops and real calls vs. inlined helpers all timed within 1 % of each other
-// (profiles/r1c_xpbd_code_size_ab.txt).  With 14-warp CTAs walking the code together (round 2) the instruction stream is fetched once
-// per CTA, and the unrolled rows win: no per-row component selects / loop control, three independent rows for the scheduler to
-// interleave - 143.7 -> 139.7 us at 4096 quadruped envs (profiles/r2j_fused_export_ab.txt), so unrolled is the default.
+// Code-size control.  The first kernel version inlined and unrolled everything and stalled on instruction fetch.  With one-warp
+// CTAs (round 1) rolled vs. unrolled 3-row joint loops and real calls vs. inlined helpers all timed about the same.
+// With wide CTAs walking the code together (round 2) the instruction stream is fetched once per CTA, and the unrolled rows win:
+// no per-row component selects / loop control, three independent rows for the scheduler to interleave, so unrolled is the default.
 // -DNB2_XPBD_ROLLED / -DNB2_XPBD_NOINLINE rebuild the other variants.
 #ifdef NB2_XPBD_NOINLINE
 #define NB2_HELPER __host__ __device__ __noinline__
@@ -519,7 +517,7 @@ enum { ST_Q = 0, ST_QD = 7, ST_COM = 13, ST_INVM = 16, ST_I = 17, ST_INVI = 26, 
 //
 // WARPS warps per CTA, each warp = 32/L environments.  All warps of a CTA walk the same code at about the same time, so the
 // 6 500-instruction iteration body (far larger than the 32 KB L1.5 instruction cache) is fetched once per CTA instead of once per
-// warp; one-warp CTAs each at their own PC were 18 % `stall_no_inst` (profiles/r1f_xpbd_step_kernel.txt).
+// warp; one-warp CTAs each at their own PC stall on instruction fetch.
 #ifndef NB2_XPBD_MIN_WARPS
 #define NB2_XPBD_MIN_WARPS 16  // resident warps per SM the register allocation must allow (16 -> 128 registers)
 #endif
@@ -1152,15 +1150,15 @@ static nb2_status launch_xpbd_W(nb2_model* m, const nb2_xpbd_params& p, const nb
         set_error("xpbd_step: environment too large for the fused shared-memory kernel (bodies per env)");
         return NB2_ERR_CAPACITY;
     }
-    // Budget: the CTAs of one SM share 227 KB (+1 KB reserved each); the batch wants >= ceil(envs / (G * 148)) resident warps per SM to
-    // stay a single wave.  The per-joint cache rides along when it does not cost that residency.
-    static const bool cache_enabled = std::getenv("NB2_XPBD_NO_JOINT_CACHE") == nullptr;  // A/B switch (profiles/r1f_xpbd_ab.txt)
+    // Budget: the CTAs of one SM share 227 KB (+1 KB reserved each); the batch wants >= ceil(envs / (G * 132)) resident warps per SM to
+    // stay a single wave on an H100 SXM.  The per-joint cache rides along when it does not cost that residency.
+    static const bool cache_enabled = std::getenv("NB2_XPBD_NO_JOINT_CACHE") == nullptr;  // A/B switch
     static const int tma_enabled = env_int("NB2_XPBD_TMA", 1), phase_sync = env_int("NB2_XPBD_PHASE_SYNC", 1);
     int flags = (tma_enabled ? XF_TMA : 0) | (phase_sync >= 1 ? XF_PHASE_SYNC : 0) | (phase_sync >= 2 ? XF_PHASE_SYNC_FINE : 0);
     XpbdPlan plan = xpbd_plan(NE, M.max_env_bodies, M.max_env_joints, contact_cap, EX, false);
     if (cache_enabled && M.d.joint_count > 0) {
         const XpbdPlan with_cache = xpbd_plan(NE, M.max_env_bodies, M.max_env_joints, contact_cap, EX, true);
-        const int want_ctas = (14 + WARPS - 1) / WARPS;  // 14 warps per SM keep 4096 two-env warps in one wave
+        const int want_ctas = (16 + WARPS - 1) / WARPS;  // 16 warps per SM keep 4096 two-env warps in one wave on 132 SMs
         if ((size_t(with_cache.total) * sizeof(float) + 1024) * want_ctas <= 227 * 1024 || size_t(plan.total) * sizeof(float) * want_ctas > 227 * 1024) {
             if (size_t(with_cache.total) * sizeof(float) <= 220 * 1024) {
                 plan = with_cache;
@@ -1172,7 +1170,7 @@ static nb2_status launch_xpbd_W(nb2_model* m, const nb2_xpbd_params& p, const nb
     int contact_cache = 0;
     {
         static const int cc_enabled = env_int("NB2_XPBD_CONTACT_CACHE", 1);
-        const int want_ctas = (14 + WARPS - 1) / WARPS;
+        const int want_ctas = (16 + WARPS - 1) / WARPS;
         const size_t budget = (size_t(227) * 1024) / want_ctas - 1024 - 64;
         const size_t base = size_t(plan.total) * sizeof(float);
         if (cc_enabled && use_contacts && base < budget) {
@@ -1188,10 +1186,10 @@ static nb2_status launch_xpbd_W(nb2_model* m, const nb2_xpbd_params& p, const nb
     }
     if (smem > 48 * 1024)
         NB2_CUDA_CHECK(cudaFuncSetAttribute(xpbd_step_kernel<L, EX, WARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
-    // ask for the largest shared-memory carve-out so that ~14-16 warps' worth of CTAs fit per SM
+    // ask for the largest shared-memory carve-out so that 16 warps' worth of CTAs fit per SM
     static const int carveout = std::getenv("NB2_XPBD_CARVEOUT") ? std::atoi(std::getenv("NB2_XPBD_CARVEOUT")) : int(cudaSharedmemCarveoutMaxShared);
     NB2_CUDA_CHECK(cudaFuncSetAttribute(xpbd_step_kernel<L, EX, WARPS>, cudaFuncAttributePreferredSharedMemoryCarveout, carveout));
-    // A/B switch: pad the grid with idle CTAs up to this many (profiles/: does a grid below the SM count change the issue rate?)
+    // A/B switch: pad the grid with idle CTAs up to this many (does a grid below the SM count change the issue rate?)
     static const int min_grid = env_int("NB2_XPBD_MIN_GRID", 0);
     const int grid = blocks < min_grid ? min_grid : blocks;
     xpbd_step_kernel<L, EX, WARPS><<<grid, 32 * WARPS, smem, s>>>(M, p, in, out, ctl, use_contacts, dt, flags, contact_cap, contact_cache);
@@ -1200,21 +1198,20 @@ static nb2_status launch_xpbd_W(nb2_model* m, const nb2_xpbd_params& p, const nb
     return NB2_OK;
 }
 
-// Warps per CTA.  Measured on B200 (profiles/r2b_xpbd_ab.txt, 4096 quadruped envs): 1 / 2 / 4 warps 166 us, 7 warps 160 us,
-// 14 warps 155 us, and 148 us with the per-iteration CTA barrier - the more warps walk the same code together, the fewer times the
-// instruction stream is fetched.  The launch takes the largest compiled width that the batch can fill on every SM
-// (14 = one CTA per SM for 4096 two-env warps), falls back when shared memory does not allow it, and honours NB2_XPBD_WARPS.
+// Warps per CTA: the more warps walk the same code together (with the per-iteration CTA barrier), the fewer times the instruction
+// stream is fetched.  The launch takes the largest compiled width that the batch can fill on every SM (16 = one CTA per SM for
+// 4096 two-env warps on the 132 SMs of an H100 SXM), falls back when shared memory does not allow it, and honours NB2_XPBD_WARPS.
 template <int L, bool EX>
 static nb2_status launch_xpbd_L(nb2_model* m, const nb2_xpbd_params& p, const nb2_state_view& in, const nb2_state_view& out,
                                 const nb2_control_view& ctl, int use_contacts, float dt, cudaStream_t s) {
     static const int forced = env_int("NB2_XPBD_WARPS", 0);
     int warps = forced;
     if (warps <= 0) {
-        int sms = 148;
+        int sms = 132;
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, m->device);
         const long long total_warps = (m->dev.env_count + (32 / L) - 1) / (32 / L);
         const long long per_sm = (total_warps + sms - 1) / sms;
-        warps = per_sm <= 1 ? 1 : (per_sm <= 4 ? 4 : 14);
+        warps = per_sm <= 1 ? 1 : (per_sm <= 4 ? 4 : 16);
     }
     // shared-memory fit (the per-CTA plan grows with the warp count)
     auto fits = [&](int w) {
@@ -1222,15 +1219,15 @@ static nb2_status launch_xpbd_L(nb2_model* m, const nb2_xpbd_params& p, const nb
         const int cap = m->contacts_imported ? m->dev.max_env_contact_slots : std::min(m->dev.max_env_contact_slots, m->max_env_contacts);
         return size_t(xpbd_plan(ne, m->dev.max_env_bodies, m->dev.max_env_joints, cap, EX, false).total) * sizeof(float) <= 200 * 1024;
     };
-    if (warps >= 14 && !fits(14)) warps = 4;
-    if (warps >= 4 && warps < 14 && !fits(4)) warps = 1;
+    if (warps >= 16 && !fits(16)) warps = 4;
+    if (warps >= 4 && warps < 16 && !fits(4)) warps = 1;
 #ifdef NB2_XPBD_AB_VARIANTS
     if constexpr (L == 16 && !EX) {
         if (warps == 2) return launch_xpbd_W<L, EX, 2>(m, p, in, out, ctl, use_contacts, dt, s);
         if (warps == 7) return launch_xpbd_W<L, EX, 7>(m, p, in, out, ctl, use_contacts, dt, s);
     }
 #endif
-    if (warps >= 14) return launch_xpbd_W<L, EX, 14>(m, p, in, out, ctl, use_contacts, dt, s);
+    if (warps >= 16) return launch_xpbd_W<L, EX, 16>(m, p, in, out, ctl, use_contacts, dt, s);
     if (warps >= 4) return launch_xpbd_W<L, EX, 4>(m, p, in, out, ctl, use_contacts, dt, s);
     return launch_xpbd_W<L, EX, 1>(m, p, in, out, ctl, use_contacts, dt, s);
 }

@@ -1,7 +1,7 @@
 """Scene construction: a compact ``ModelBuilder`` producing :class:`newton_b200.Model` arrays.
 
 Scope note (SURVEY.md §2 row 5, §8(b)): the reference's 13 kLoC ``ModelBuilder`` is host-side
-model construction that runs once and is *out of scope* for the B200 hot path; a user of the
+model construction that runs once and is *out of scope* for the GPU hot path; a user of the
 reference keeps using it.  This module exists because the reference builder cannot be imported
 without Warp, and the parity tests / benchmark need bit-identical ``Model`` inputs for the oracle
 and the CUDA path.  It mirrors the subset of the reference API that the BASELINE.json configs

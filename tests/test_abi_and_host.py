@@ -23,7 +23,7 @@ def test_library_exports_every_declared_symbol():
     L = _lib.lib()
     for sym in declared:
         assert hasattr(L, sym), sym
-    assert b"sm_100a" in L.nb2_version()
+    assert b"sm_90a" in L.nb2_version()
 
 
 def test_abi_struct_matches_header_field_order():
