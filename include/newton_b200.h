@@ -306,6 +306,41 @@ nb2_status nb2_eval_fk_masked(nb2_model* model, const float* joint_q, const floa
                               const uint8_t* articulation_mask, const int32_t* articulation_indices, int32_t index_count,
                               int32_t body_flag_filter, void* cuda_stream);
 
+/* --- articulation dynamics queries (one warp per articulation, intermediates in shared memory) -----------------------------
+ * Joint-space quantities of every articulation tree (joints articulation_start[a] .. articulation_end[a]; loop-closing joints
+ * play no part, as upstream).  Inputs are State arrays (body_q must already reflect joint_q, e.g. after nb2_eval_fk); outputs
+ * use the reference layouts: J [articulation_count, 6 max_links, max_dofs], H [articulation_count, max_dofs, max_dofs] (both
+ * row-major, padding rows / columns written as 0), forces [joint_dof_count] in the Control.joint_f convention.
+ * `articulation_mask` ([articulation_count] bytes, 0 = skip) may be NULL; skipped articulations get zero outputs.
+ * max_links / max_dofs are the output layout (Model.max_joints_per_articulation / max_dofs_per_articulation) and must cover the
+ * largest articulation.  An articulation too large for the kernels' per-warp shared memory fails with NB2_ERR_CAPACITY
+ * (DESIGN.md section 7).  No call allocates or synchronises: with caller-provided outputs each is graph-capturable. */
+
+/* Reference newton.eval_jacobian (sim/articulation.py:934-1248): J[a][6 i + k][col] is the world, COM-referenced twist of link i
+ * (the child of the articulation's i-th joint) per unit joint_qd[col], so J_link @ joint_qd == body_qd[link]. */
+nb2_status nb2_eval_jacobian(nb2_model* model, const float* body_q, const float* joint_q, float* J, int32_t max_links, int32_t max_dofs,
+                             const uint8_t* articulation_mask, void* cuda_stream);
+
+/* Reference newton.eval_mass_matrix (sim/articulation.py:1251-1376, 1593-1690): H = sum over links of J_i^T I_i J_i with the world
+ * COM inertia I_i = blockdiag(m 1, R I R^T).  `J` may be NULL (the Jacobian is formed in shared memory and not written out) or
+ * the caller's Jacobian in the layout above, which is then read instead. */
+nb2_status nb2_eval_mass_matrix(nb2_model* model, const float* body_q, const float* joint_q, const float* J, float* H, int32_t max_links,
+                                int32_t max_dofs, const uint8_t* articulation_mask, void* cuda_stream);
+
+/* Reference newton.eval_inverse_dynamics_passive (sim/inverse_dynamics.py:364-485): whichever of M(q) (`mass_matrix`, as
+ * nb2_eval_mass_matrix), g(q) (`gravity_force`, an RNEA pass with joint_qd = 0 under model.gravity) and C(q, qd) qd
+ * (`coriolis_force`, an RNEA pass with `joint_qd` and zero gravity) are non-NULL, in one launch; at least one must be.  The two
+ * RNEA passes follow _rnea_compensation_pass (:113-308; featherstone/kernels.py:925, 1242, 1321, 1092). */
+nb2_status nb2_eval_inverse_dynamics_passive(nb2_model* model, const float* body_q, const float* joint_q, const float* joint_qd,
+                                             float* mass_matrix, float* gravity_force, float* coriolis_force, int32_t max_dofs,
+                                             const uint8_t* articulation_mask, void* cuda_stream);
+
+/* Reference newton.eval_inverse_dynamics_force (sim/articulation.py:1379-1590): joint_f = M qdd + C qd + g, the M qdd part of every
+ * FREE/DISTANCE joint rotated from its parent frame into the world frame; loop-closure dofs after an articulation's tree are 0. */
+nb2_status nb2_eval_inverse_dynamics_force(nb2_model* model, const float* body_q, const float* mass_matrix, const float* joint_qdd,
+                                           const float* coriolis_force, const float* gravity_force, float* joint_f, int32_t max_dofs,
+                                           const uint8_t* articulation_mask, void* cuda_stream);
+
 /* --- ArticulationView attribute access (SURVEY.md §8(f) rank 2) -------------------------------------------------------
  * Reference newton.selection.ArticulationView (utils/selection.py): `_get_attribute_array` (:1232-1357) views an attribute
  * array as [world, articulation, value, trailing...] through an offset and two strides; `_get_attribute_values`

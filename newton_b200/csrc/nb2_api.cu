@@ -285,6 +285,17 @@ static nb2_status build_tables(nb2_model* m, const nb2_model_desc& d) {
                 }
             }
         }
+        // ---- articulation trees of the public dynamics calls (nb2_dynamics.cu): joints [start, articulation_end), i.e. the leading
+        // joints whose joint_articulation is the articulation; later joints of the range close loops
+        h.tree_max_joints = h.tree_max_dofs = 0;
+        h.has_rod = false;
+        for (int j = 0; j < J; ++j) h.has_rod = h.has_rod || jtype[j] == 7;  // JointType.ROD
+        for (int a = 0; a < d.articulation_count; ++a) {
+            int je = art_start[a];
+            while (je < art_start[a + 1] && jart[je] == a) ++je;
+            h.tree_max_joints = std::max(h.tree_max_joints, je - art_start[a]);
+            h.tree_max_dofs = std::max(h.tree_max_dofs, jqd[je] - jqd[art_start[a]]);
+        }
         // ---- H-stage schedule (see DevModel): the per-(depth, dof number) column batches of every articulation ----------------
         h.joint_desc_mask.assign(size_t(J), 0ull);
         h.dof_joint.assign(size_t(jqd[J]), 0);
@@ -842,6 +853,63 @@ nb2_status nb2_eval_ik(nb2_model* model, const float* body_q, const float* body_
     }
     DeviceGuard guard(model->device);
     return launch_eval_ik(model, body_q, body_qd, joint_q, joint_qd, static_cast<cudaStream_t>(cuda_stream));
+}
+
+nb2_status nb2_eval_jacobian(nb2_model* model, const float* body_q, const float* joint_q, float* J, int32_t max_links, int32_t max_dofs,
+                             const uint8_t* articulation_mask, void* cuda_stream) {
+    if (!model || !body_q || !joint_q || (!J && model->dev.d.articulation_count > 0)) {
+        set_error("nb2_eval_jacobian: NULL argument");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    DeviceGuard guard(model->device);
+    return launch_eval_jacobian(model, body_q, joint_q, J, max_links, max_dofs, articulation_mask, static_cast<cudaStream_t>(cuda_stream));
+}
+
+nb2_status nb2_eval_mass_matrix(nb2_model* model, const float* body_q, const float* joint_q, const float* J, float* H, int32_t max_links,
+                                int32_t max_dofs, const uint8_t* articulation_mask, void* cuda_stream) {
+    if (!model || !body_q || !joint_q || (!H && model->dev.d.articulation_count > 0)) {
+        set_error("nb2_eval_mass_matrix: NULL argument");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    DeviceGuard guard(model->device);
+    return launch_eval_mass_matrix(model, body_q, joint_q, J, H, max_links, max_dofs, articulation_mask, static_cast<cudaStream_t>(cuda_stream));
+}
+
+nb2_status nb2_eval_inverse_dynamics_passive(nb2_model* model, const float* body_q, const float* joint_q, const float* joint_qd,
+                                             float* mass_matrix, float* gravity_force, float* coriolis_force, int32_t max_dofs,
+                                             const uint8_t* articulation_mask, void* cuda_stream) {
+    if (!model || !body_q || !joint_q || (coriolis_force && !joint_qd)) {
+        set_error("nb2_eval_inverse_dynamics_passive: NULL argument");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    if (!mass_matrix && !gravity_force && !coriolis_force) {
+        set_error("nb2_eval_inverse_dynamics_passive: at least one inverse-dynamics output must be provided");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    if (model->host.has_rod) {
+        set_error("nb2_eval_inverse_dynamics_passive: JointType.ROD joints are not supported");
+        return NB2_ERR_UNSUPPORTED;
+    }
+    DeviceGuard guard(model->device);
+    return launch_eval_inverse_dynamics_passive(model, body_q, joint_q, joint_qd, mass_matrix, gravity_force, coriolis_force, max_dofs,
+                                                articulation_mask, static_cast<cudaStream_t>(cuda_stream));
+}
+
+nb2_status nb2_eval_inverse_dynamics_force(nb2_model* model, const float* body_q, const float* mass_matrix, const float* joint_qdd,
+                                           const float* coriolis_force, const float* gravity_force, float* joint_f, int32_t max_dofs,
+                                           const uint8_t* articulation_mask, void* cuda_stream) {
+    if (!model || !body_q || (model->dev.d.articulation_count > 0 && model->dev.d.joint_dof_count > 0 &&
+                              (!mass_matrix || !joint_qdd || !coriolis_force || !gravity_force || !joint_f))) {
+        set_error("nb2_eval_inverse_dynamics_force: NULL argument");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    if (model->host.has_rod) {
+        set_error("nb2_eval_inverse_dynamics_force: JointType.ROD joints are not supported");
+        return NB2_ERR_UNSUPPORTED;
+    }
+    DeviceGuard guard(model->device);
+    return launch_eval_inverse_dynamics_force(model, body_q, mass_matrix, joint_qdd, coriolis_force, gravity_force, joint_f, max_dofs,
+                                              articulation_mask, static_cast<cudaStream_t>(cuda_stream));
 }
 
 const char* nb2_last_error(void) { return g_last_error.c_str(); }

@@ -106,6 +106,8 @@ struct HostTables {
     int max_art_dofs = 0;  // largest articulation (dofs)
     bool featherstone_supported = true;
     bool fk_levels = true;     // eval_fk may schedule joints by tree depth (parent-before-child order, one driving joint per body)
+    int tree_max_joints = 0, tree_max_dofs = 0;  // largest articulation tree (joints / dofs up to articulation_end)
+    bool has_rod = false;      // some joint is a ROD (refused by the inverse-dynamics calls, like upstream)
     std::string featherstone_reason;
 };
 
@@ -168,6 +170,14 @@ nb2_status launch_eval_fk(nb2_model* m, const float* joint_q, const float* joint
                           cudaStream_t s, const uint8_t* mask = nullptr, const int* indices = nullptr, int index_count = 0,
                           int body_flag_filter = 3);
 nb2_status launch_eval_ik(nb2_model* m, const float* body_q, const float* body_qd, float* joint_q, float* joint_qd, cudaStream_t s);
+nb2_status launch_eval_jacobian(nb2_model* m, const float* body_q, const float* joint_q, float* J, int max_links, int max_dofs,
+                                const uint8_t* mask, cudaStream_t s);
+nb2_status launch_eval_mass_matrix(nb2_model* m, const float* body_q, const float* joint_q, const float* J, float* H, int max_links,
+                                   int max_dofs, const uint8_t* mask, cudaStream_t s);
+nb2_status launch_eval_inverse_dynamics_passive(nb2_model* m, const float* body_q, const float* joint_q, const float* joint_qd, float* H,
+                                                float* gravity_force, float* coriolis_force, int max_dofs, const uint8_t* mask, cudaStream_t s);
+nb2_status launch_eval_inverse_dynamics_force(nb2_model* m, const float* body_q, const float* H, const float* joint_qdd, const float* coriolis_force,
+                                              const float* gravity_force, float* joint_f, int max_dofs, const uint8_t* mask, cudaStream_t s);
 }  // namespace nb2
 
 #define NB2_CUDA_CHECK(expr)                                                                          \

@@ -564,3 +564,31 @@ class ArticulationView:
         from .sim.articulation import eval_fk
 
         eval_fk(self.model, target.joint_q, target.joint_qd, target, mask=self.get_model_articulation_mask(mask=mask))
+
+    def eval_jacobian(self, state, J=None, joint_S_s=None, mask=None):
+        """:func:`newton_b200.eval_jacobian` of the selected articulations (reference ``selection.py:1774-1792``); ``mask`` is a
+        view mask ``(world_count,)`` or ``(world_count, count_per_world)``."""
+        from .sim.articulation import eval_jacobian
+
+        return eval_jacobian(self.model, state, J, joint_S_s=joint_S_s, mask=self.get_model_articulation_mask(mask=mask))
+
+    def eval_mass_matrix(self, state, H=None, J=None, body_I_s=None, joint_S_s=None, mask=None):
+        """:func:`newton_b200.eval_mass_matrix` of the selected articulations (reference ``selection.py:1794-1817``)."""
+        from .sim.articulation import eval_mass_matrix
+
+        return eval_mass_matrix(self.model, state, H, J=J, body_I_s=body_I_s, joint_S_s=joint_S_s,
+                                mask=self.get_model_articulation_mask(mask=mask))
+
+    def eval_inverse_dynamics_passive(self, state, *, mass_matrix=None, gravity_force=None, coriolis_force=None, mask=None) -> None:
+        """:func:`newton_b200.eval_inverse_dynamics_passive` of the selected articulations (reference ``selection.py:1819-1867``)."""
+        from .sim.articulation import eval_inverse_dynamics_passive
+
+        eval_inverse_dynamics_passive(self.model, state, mass_matrix=mass_matrix, gravity_force=gravity_force,
+                                      coriolis_force=coriolis_force, mask=self.get_model_articulation_mask(mask=mask))
+
+    def eval_inverse_dynamics_force(self, state, *, mass_matrix, joint_qdd, coriolis_force, gravity_force, joint_f, mask=None) -> None:
+        """:func:`newton_b200.eval_inverse_dynamics_force` of the selected articulations (reference ``selection.py:1869-1921``)."""
+        from .sim.articulation import eval_inverse_dynamics_force
+
+        eval_inverse_dynamics_force(self.model, state, mass_matrix=mass_matrix, joint_qdd=joint_qdd, coriolis_force=coriolis_force,
+                                    gravity_force=gravity_force, joint_f=joint_f, mask=self.get_model_articulation_mask(mask=mask))

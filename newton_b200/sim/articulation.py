@@ -80,3 +80,183 @@ def eval_ik(model, state, joint_q, joint_qd) -> None:
                 _lib.current_stream_ptr(model)),
             "nb2_eval_ik",
         )
+
+
+# ---- articulation dynamics queries: newton.eval_jacobian / eval_mass_matrix / eval_inverse_dynamics_passive / _force -------------
+# The kernels (csrc/nb2_dynamics.cu) run one warp per articulation and keep every intermediate in shared memory, so a call is one
+# launch with no allocation and no host synchronisation once its outputs exist.  Argument checks happen before the CUDA-only
+# check, with the reference's messages.
+
+
+def _has_rod(model) -> bool:
+    cached = getattr(model, "_nb2_has_rod", None)
+    if cached is None:
+        from .enums import JointType
+
+        cached = bool((model.numpy("joint_type") == int(JointType.ROD)).any()) if int(model.joint_count) else False
+        model._nb2_has_rod = cached
+    return cached
+
+
+def _check_shape(name, array, expected):
+    if array is not None and tuple(array.shape) != tuple(expected):
+        raise ValueError(f"{name} has shape {tuple(array.shape)}, expected {tuple(expected)}.")
+
+
+def _native_call(model, what):
+    from .. import _lib
+
+    if not torch.device(model.device).type == "cuda":
+        raise _lib.Nb2Error(f"newton_b200.{what} runs on CUDA devices only (no CPU path); CPU checks use oracle.dynamics "
+                            "(test infrastructure).")
+    return _lib.native_model(model)
+
+
+def _mask_ptr(mask, model):
+    import ctypes as C
+
+    from .. import _abi
+
+    return C.c_void_p(_abi.ptr(mask, "bool", model.device, int(model.articulation_count), "mask"))
+
+
+def _jacobian_shape(model):
+    return (int(model.articulation_count), 6 * int(model.max_joints_per_articulation), int(model.max_dofs_per_articulation))
+
+
+def _mass_matrix_shape(model):
+    return (int(model.articulation_count), int(model.max_dofs_per_articulation), int(model.max_dofs_per_articulation))
+
+
+def eval_jacobian(model, state, J=None, joint_S_s=None, mask=None):
+    """Spatial Jacobian of every articulation (reference ``newton.eval_jacobian``, ``sim/articulation.py:1171-1248``).
+
+    Returns ``J`` of shape ``(articulation_count, 6 * max_joints_per_articulation, max_dofs_per_articulation)`` with
+    ``J[a, 6 i : 6 i + 6] @ joint_qd == state.body_qd[link]`` for the child of the articulation's i-th joint (COM-referenced world
+    twists), or ``None`` when the model has no articulations.  ``J`` is allocated when omitted; every entry is written, padding and
+    masked-out articulations (``mask``, bool ``[articulation_count]``) as 0.  ``joint_S_s`` is accepted for calls written
+    against the reference, where it is a temporary; the kernel keeps the motion subspaces in shared memory and never writes it.
+    Reads ``state.body_q`` and ``state.joint_q``.
+    """
+    if int(model.articulation_count) == 0:
+        return None
+    _check_shape("J", J, _jacobian_shape(model))
+    _check_shape("mask", mask, (int(model.articulation_count),))
+    nm = _native_call(model, "eval_jacobian")
+    import ctypes as C
+
+    from .. import _abi, _lib
+
+    if J is None:
+        J = torch.empty(_jacobian_shape(model), dtype=torch.float32, device=model.device)
+    dev = model.device
+    with torch.cuda.device(nm.device_index):
+        _lib.check(_lib.lib().nb2_eval_jacobian(
+            nm.handle, C.c_void_p(_abi.ptr(state.body_q, "f32", dev, 7 * int(model.body_count), "state.body_q")),
+            C.c_void_p(_abi.ptr(state.joint_q, "f32", dev, int(model.joint_coord_count), "state.joint_q")),
+            C.c_void_p(_abi.ptr(J, "f32", dev, J.numel(), "J")), int(model.max_joints_per_articulation), int(model.max_dofs_per_articulation),
+            _mask_ptr(mask, model), _lib.current_stream_ptr(model)), "nb2_eval_jacobian")
+    return J
+
+
+def eval_mass_matrix(model, state, H=None, J=None, body_I_s=None, joint_S_s=None, mask=None):
+    """Generalized mass matrix ``H = J^T M J`` of every articulation (reference ``newton.eval_mass_matrix``,
+    ``sim/articulation.py:1593-1690``), consistent with the kinetic energy of the COM-referenced body twists.
+
+    Returns ``H`` of shape ``(articulation_count, max_dofs_per_articulation, max_dofs_per_articulation)`` (allocated when omitted;
+    padding and masked-out articulations are 0), or ``None`` without articulations.  With ``J`` given, that Jacobian is read
+    instead of being formed; without it the Jacobian lives in shared memory only.  ``body_I_s`` and ``joint_S_s`` are accepted
+    for calls written against the reference, where they are temporaries; they are never written.
+    """
+    if int(model.articulation_count) == 0:
+        return None
+    _check_shape("H", H, _mass_matrix_shape(model))
+    _check_shape("J", J, _jacobian_shape(model))
+    _check_shape("mask", mask, (int(model.articulation_count),))
+    nm = _native_call(model, "eval_mass_matrix")
+    import ctypes as C
+
+    from .. import _abi, _lib
+
+    if H is None:
+        H = torch.empty(_mass_matrix_shape(model), dtype=torch.float32, device=model.device)
+    dev = model.device
+    with torch.cuda.device(nm.device_index):
+        _lib.check(_lib.lib().nb2_eval_mass_matrix(
+            nm.handle, C.c_void_p(_abi.ptr(state.body_q, "f32", dev, 7 * int(model.body_count), "state.body_q")),
+            C.c_void_p(_abi.ptr(state.joint_q, "f32", dev, int(model.joint_coord_count), "state.joint_q")),
+            C.c_void_p(None if J is None else _abi.ptr(J, "f32", dev, J.numel(), "J")),
+            C.c_void_p(_abi.ptr(H, "f32", dev, H.numel(), "H")), int(model.max_joints_per_articulation),
+            int(model.max_dofs_per_articulation), _mask_ptr(mask, model), _lib.current_stream_ptr(model)), "nb2_eval_mass_matrix")
+    return H
+
+
+def eval_inverse_dynamics_passive(model, state, *, mass_matrix=None, gravity_force=None, coriolis_force=None, mask=None) -> None:
+    """Passive inverse-dynamics terms (reference ``newton.eval_inverse_dynamics_passive``, ``sim/inverse_dynamics.py:364-485``).
+
+    Each non-``None`` output is computed, all in one launch: ``mass_matrix`` <- ``M(q)`` (as :func:`eval_mass_matrix`),
+    ``gravity_force`` <- ``g(q) = dU/dq`` and ``coriolis_force`` <- ``C(q, qd) qd``, following ``tau = M qdd + C qd + g``.  The
+    two force terms come from two separate RNEA passes (joint_qd = 0 under ``model.gravity``; ``state.joint_qd`` under zero
+    gravity).  ``state.body_q`` must already reflect ``state.joint_q`` (call :func:`eval_fk` first).  Entries of articulations
+    that ``mask`` leaves out are 0.  Loop-closure joints play no part; ROD joints are refused.
+    """
+    if _has_rod(model):
+        raise ValueError("eval_inverse_dynamics_passive() does not support JointType.ROD joints.")
+    if mass_matrix is None and gravity_force is None and coriolis_force is None:
+        raise ValueError("At least one inverse-dynamics output must be provided.")
+    _check_shape("mass_matrix", mass_matrix, _mass_matrix_shape(model))
+    for name, array in (("gravity_force", gravity_force), ("coriolis_force", coriolis_force)):
+        _check_shape(name, array, (int(model.joint_dof_count),))
+    _check_shape("mask", mask, (int(model.articulation_count),))
+    if int(model.articulation_count) == 0:
+        return
+    nm = _native_call(model, "eval_inverse_dynamics_passive")
+    import ctypes as C
+
+    from .. import _abi, _lib
+
+    dev, nd = model.device, int(model.joint_dof_count)
+
+    def out(a, name):
+        return C.c_void_p(None if a is None else _abi.ptr(a, "f32", dev, a.numel(), name))
+
+    with torch.cuda.device(nm.device_index):
+        _lib.check(_lib.lib().nb2_eval_inverse_dynamics_passive(
+            nm.handle, C.c_void_p(_abi.ptr(state.body_q, "f32", dev, 7 * int(model.body_count), "state.body_q")),
+            C.c_void_p(_abi.ptr(state.joint_q, "f32", dev, int(model.joint_coord_count), "state.joint_q")),
+            C.c_void_p(_abi.ptr(state.joint_qd, "f32", dev, nd, "state.joint_qd")), out(mass_matrix, "mass_matrix"),
+            out(gravity_force, "gravity_force"), out(coriolis_force, "coriolis_force"), int(model.max_dofs_per_articulation),
+            _mask_ptr(mask, model), _lib.current_stream_ptr(model)), "nb2_eval_inverse_dynamics_passive")
+
+
+def eval_inverse_dynamics_force(model, state, *, mass_matrix, joint_qdd, coriolis_force, gravity_force, joint_f, mask=None) -> None:
+    """``joint_f = M(q) qdd + C(q, qd) qd + g(q)`` (reference ``newton.eval_inverse_dynamics_force``,
+    ``sim/articulation.py:1471-1590``), in the ``Control.joint_f`` convention: the ``M qdd`` part of every FREE/DISTANCE joint is
+    rotated from its parent frame into the world frame with ``state.body_q``.  Dofs of articulations that ``mask`` leaves out and
+    loop-closure dofs after an articulation's tree are set to 0.  ROD joints are refused.
+    """
+    if _has_rod(model):
+        raise ValueError("eval_inverse_dynamics_force() does not support JointType.ROD joints.")
+    if int(model.articulation_count) == 0:
+        return
+    _check_shape("mass_matrix", mass_matrix, _mass_matrix_shape(model))
+    for name, array in (("joint_qdd", joint_qdd), ("coriolis_force", coriolis_force), ("gravity_force", gravity_force),
+                        ("joint_f", joint_f)):
+        _check_shape(name, array, (int(model.joint_dof_count),))
+    _check_shape("mask", mask, (int(model.articulation_count),))
+    nm = _native_call(model, "eval_inverse_dynamics_force")
+    import ctypes as C
+
+    from .. import _abi, _lib
+
+    dev, nd = model.device, int(model.joint_dof_count)
+
+    def arg(a, name):
+        return C.c_void_p(_abi.ptr(a, "f32", dev, a.numel(), name))
+
+    with torch.cuda.device(nm.device_index):
+        _lib.check(_lib.lib().nb2_eval_inverse_dynamics_force(
+            nm.handle, C.c_void_p(_abi.ptr(state.body_q, "f32", dev, 7 * int(model.body_count), "state.body_q")),
+            arg(mass_matrix, "mass_matrix"), arg(joint_qdd, "joint_qdd"), arg(coriolis_force, "coriolis_force"),
+            arg(gravity_force, "gravity_force"), arg(joint_f, "joint_f"), int(model.max_dofs_per_articulation), _mask_ptr(mask, model),
+            _lib.current_stream_ptr(model)), "nb2_eval_inverse_dynamics_force")
