@@ -398,6 +398,45 @@ typedef struct nb2_match_options {
 nb2_status nb2_contacts_match(nb2_model* model, const float* body_q, const nb2_contacts_view* contacts, int32_t* match_index,
                               const nb2_match_options* options, void* cuda_stream);
 
+/* --- contact sensor (reference newton.sensors.SensorContact, sensors/sensor_contact.py) -----------------------------------
+ * Sums Contacts.force per sensing object (row) and, optionally, per counterpart (column).  The row / column maps are built by
+ * the caller (newton_b200.sensors.SensorContact, on the host) and already expanded from bodies to shapes: shape_to_row /
+ * shape_to_col hold one entry per shape, -1 where the shape is not sensed / not a counterpart.  Every output entry is the sum
+ * of its contributions in ascending contact index, the shape0 side of a contact before its shape1 side, whatever order the
+ * contacts sit in: the reference's serial order, reproduced without float atomics.  A contact whose shape id lies outside
+ * [0, shape_count) contributes nothing.  The library keeps no per-sensor state; the caller owns the outputs and a scratch
+ * buffer of nb2_sensor_contact_scratch_bytes() bytes, so an update allocates nothing, does not synchronise and can be captured
+ * into a CUDA graph.  Launch order: one thread per contact slot (force, friction, weighted midpoint, two sort records), a
+ * stable radix sort of the records by row, memsets of the matrices, one thread per row summing its run in order. */
+typedef struct nb2_sensor_contact_view {
+    int32_t shape_count;
+    int32_t row_count;           /* sensing objects */
+    int32_t col_count;           /* counterpart columns (max over worlds); 0 = no per-counterpart outputs */
+    int32_t sensing_kind;        /* NB2_SENSING_SHAPE or NB2_SENSING_BODY */
+    const int32_t* shape_to_row; /* [shape_count] */
+    const int32_t* shape_to_col; /* [shape_count]; may be NULL when col_count == 0 */
+    const int32_t* sensing_indices; /* [row_count] body or shape index of each row */
+    const int32_t* shape_body;      /* Model.shape_body */
+    const float* shape_transform;   /* Model.shape_transform */
+    float* total_force;             /* vec3[row_count] or NULL; total_force_friction likewise (both or neither) */
+    float* total_force_friction;
+    float* force_matrix;            /* vec3[row_count, col_count]; the three matrices are all set iff col_count > 0 */
+    float* force_matrix_friction;
+    float* position_matrix;
+    float* sensing_transforms;      /* transform[row_count]; written only when body_q is given */
+} nb2_sensor_contact_view;
+
+enum { NB2_SENSING_SHAPE = 1, NB2_SENSING_BODY = 2 };
+
+/* Scratch bytes one update needs for a Contacts buffer of `rigid_contact_max` slots and the sensor's layout. */
+nb2_status nb2_sensor_contact_scratch_bytes(int32_t rigid_contact_max, int32_t row_count, int32_t col_count, size_t* bytes);
+
+/* Reference SensorContact.update (sensors/sensor_contact.py:684-775).  `contacts` needs rigid_contact_count, shape0, shape1,
+ * normal and force, and point0 / point1 / offset0 / offset1 when positions are computed.  `body_q` may be NULL: the positions are
+ * then written as 0 and sensing_transforms is left unchanged.  Every output the sensor has is overwritten in full. */
+nb2_status nb2_sensor_contact_update(const nb2_sensor_contact_view* sensor, const nb2_contacts_view* contacts, const float* body_q,
+                                     void* scratch, size_t scratch_bytes, void* cuda_stream);
+
 /* --- multi-GPU end-of-frame state gather without compute kernels (SURVEY.md §8(e)) --------------------------------------
  * Replaces the `ncclAllGather(body_q, body_qd)` of the reference design (there is no reference code for it: upstream is
  * single-GPU; the sharding follows sim/model.py:1081-1097 world ranges).  Every rank owns a receive buffer of

@@ -7,3 +7,4 @@ from .sim import (  # noqa: F401
 from .sim.collide import CollisionPipeline, SpeculativeContactConfig  # noqa: F401,E402
 from . import solvers  # noqa: F401,E402
 from . import selection  # noqa: F401,E402
+from . import sensors  # noqa: F401,E402

@@ -210,6 +210,19 @@ class MatchOptions(C.Structure):
                 ("broken_count", C.c_void_p)]
 
 
+class SensorContactView(C.Structure):
+    """``nb2_sensor_contact_view``"""
+
+    _fields_ = [("shape_count", C.c_int32), ("row_count", C.c_int32), ("col_count", C.c_int32), ("sensing_kind", C.c_int32),
+                ("shape_to_row", C.c_void_p), ("shape_to_col", C.c_void_p), ("sensing_indices", C.c_void_p), ("shape_body", C.c_void_p),
+                ("shape_transform", C.c_void_p), ("total_force", C.c_void_p), ("total_force_friction", C.c_void_p),
+                ("force_matrix", C.c_void_p), ("force_matrix_friction", C.c_void_p), ("position_matrix", C.c_void_p),
+                ("sensing_transforms", C.c_void_p)]
+
+
+SENSING_SHAPE, SENSING_BODY = 1, 2  # NB2_SENSING_* (the reference's _SENSING_KIND_* values)
+
+
 class FeatherstoneParams(C.Structure):
     _fields_ = [
         ("angular_damping", C.c_float),

@@ -28,6 +28,7 @@ EXPORTED_SYMBOLS = (
     "nb2_model_create", "nb2_model_destroy", "nb2_model_notify_changed", "nb2_model_rigid_contact_max", "nb2_collide_configure", "nb2_collide", "nb2_collide_speculative", "nb2_contacts_match", "nb2_contacts_sort", "nb2_contacts_import",
     "nb2_xpbd_step", "nb2_xpbd_update_contacts", "nb2_integrate_bodies", "nb2_featherstone_step", "nb2_eval_fk", "nb2_eval_ik", "nb2_eval_fk_masked",
     "nb2_eval_jacobian", "nb2_eval_mass_matrix", "nb2_eval_inverse_dynamics_passive", "nb2_eval_inverse_dynamics_force",
+    "nb2_sensor_contact_scratch_bytes", "nb2_sensor_contact_update",
     "nb2_view_gather", "nb2_view_scatter", "nb2_view_articulation_mask", "nb2_last_error", "nb2_kernel_launch_count", "nb2_version",
     "nb2_peer_gather_handle_bytes", "nb2_peer_gather_create", "nb2_peer_gather_buffer", "nb2_peer_gather_stride", "nb2_peer_gather_export",
     "nb2_peer_gather_connect", "nb2_peer_gather_push", "nb2_peer_gather_wait", "nb2_peer_gather_destroy",
@@ -93,6 +94,10 @@ def lib():
         L.nb2_eval_inverse_dynamics_passive.restype = C.c_int
         L.nb2_eval_inverse_dynamics_force.argtypes = [P, P, P, P, P, P, P, C.c_int32, P, P]
         L.nb2_eval_inverse_dynamics_force.restype = C.c_int
+        L.nb2_sensor_contact_scratch_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_size_t)]
+        L.nb2_sensor_contact_scratch_bytes.restype = C.c_int
+        L.nb2_sensor_contact_update.argtypes = [C.POINTER(_abi.SensorContactView), C.POINTER(_abi.ContactsView), P, P, C.c_size_t, P]
+        L.nb2_sensor_contact_update.restype = C.c_int
         L.nb2_view_gather.argtypes = [P, C.POINTER(_abi.ViewLayout), P, P]
         L.nb2_view_gather.restype = C.c_int
         L.nb2_view_scatter.argtypes = [P, C.POINTER(_abi.ViewLayout), P, P, C.c_int32, P]

@@ -14,7 +14,7 @@ LIB = os.path.join(HERE, "libnewton_b200.so")
 # north-star tolerance instead of bit equality (tests/test_gpu_fast_fp.py).
 LIB_FAST = os.path.join(HERE, "libnewton_b200_fast.so")
 STRICT_FLAGS = ["-fmad=false", "-DNB2_STRICT_FP=1"]
-SOURCES = ["nb2_api.cu", "nb2_collide.cu", "nb2_xpbd.cu", "nb2_featherstone.cu", "nb2_dynamics.cu", "nb2_selection.cu", "nb2_peer.cu", "nb2_match.cu"]
+SOURCES = ["nb2_api.cu", "nb2_collide.cu", "nb2_xpbd.cu", "nb2_featherstone.cu", "nb2_dynamics.cu", "nb2_sensor.cu", "nb2_selection.cu", "nb2_peer.cu", "nb2_match.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--expt-relaxed-constexpr",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-O2",

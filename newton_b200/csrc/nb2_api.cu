@@ -912,6 +912,57 @@ nb2_status nb2_eval_inverse_dynamics_force(nb2_model* model, const float* body_q
                                               articulation_mask, static_cast<cudaStream_t>(cuda_stream));
 }
 
+nb2_status nb2_sensor_contact_scratch_bytes(int32_t rigid_contact_max, int32_t row_count, int32_t col_count, size_t* bytes) {
+    if (!bytes || rigid_contact_max < 0 || row_count < 0 || col_count < 0 || rigid_contact_max > (1 << 29)) {
+        set_error("nb2_sensor_contact_scratch_bytes: invalid argument");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    return sensor_contact_scratch_bytes(rigid_contact_max, row_count, col_count, bytes);
+}
+
+nb2_status nb2_sensor_contact_update(const nb2_sensor_contact_view* sensor, const nb2_contacts_view* contacts, const float* body_q,
+                                     void* scratch, size_t scratch_bytes, void* cuda_stream) {
+    if (!sensor || !contacts || (!scratch && scratch_bytes > 0)) {
+        set_error("nb2_sensor_contact_update: NULL argument");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    const nb2_sensor_contact_view& s = *sensor;
+    const nb2_contacts_view& c = *contacts;
+    if (s.shape_count < 0 || s.row_count < 0 || s.col_count < 0 || c.rigid_contact_max < 0 || c.rigid_contact_max > (1 << 29) ||
+        (s.sensing_kind != NB2_SENSING_SHAPE && s.sensing_kind != NB2_SENSING_BODY)) {
+        set_error("nb2_sensor_contact_update: invalid counts or sensing_kind");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    if (s.row_count > 0 && (!s.sensing_indices || !s.sensing_transforms || (s.shape_count > 0 && (!s.shape_to_row || !s.shape_body ||
+                                                                                                  !s.shape_transform)))) {
+        set_error("nb2_sensor_contact_update: sensor layout arrays are NULL");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    if (!s.total_force != !s.total_force_friction) {
+        set_error("nb2_sensor_contact_update: total_force and total_force_friction must both be given or both be NULL");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    if (s.col_count > 0 && (!s.force_matrix || !s.force_matrix_friction || !s.position_matrix || (s.shape_count > 0 && !s.shape_to_col))) {
+        set_error("nb2_sensor_contact_update: col_count > 0 needs force_matrix, force_matrix_friction, position_matrix and shape_to_col");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    if (c.rigid_contact_max > 0) {
+        if (!c.force) {
+            set_error("nb2_sensor_contact_update: contacts.force is NULL");
+            return NB2_ERR_INVALID_ARGUMENT;
+        }
+        if (!c.rigid_contact_count || !c.shape0 || !c.shape1 || !c.normal) {
+            set_error("nb2_sensor_contact_update: contacts view has NULL arrays");
+            return NB2_ERR_INVALID_ARGUMENT;
+        }
+        if (body_q && s.col_count > 0 && (!c.point0 || !c.point1 || !c.offset0 || !c.offset1)) {
+            set_error("nb2_sensor_contact_update: contact positions need point0, point1, offset0 and offset1");
+            return NB2_ERR_INVALID_ARGUMENT;
+        }
+    }
+    return launch_sensor_contact_update(s, c, body_q, scratch, scratch_bytes, static_cast<cudaStream_t>(cuda_stream));
+}
+
 const char* nb2_last_error(void) { return g_last_error.c_str(); }
 int64_t nb2_kernel_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
 const char* nb2_version(void) { return "newton_b200 0.1 (sm_90a)"; }

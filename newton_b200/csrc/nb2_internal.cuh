@@ -178,6 +178,9 @@ nb2_status launch_eval_inverse_dynamics_passive(nb2_model* m, const float* body_
                                                 float* gravity_force, float* coriolis_force, int max_dofs, const uint8_t* mask, cudaStream_t s);
 nb2_status launch_eval_inverse_dynamics_force(nb2_model* m, const float* body_q, const float* H, const float* joint_qdd, const float* coriolis_force,
                                               const float* gravity_force, float* joint_f, int max_dofs, const uint8_t* mask, cudaStream_t s);
+nb2_status sensor_contact_scratch_bytes(int rigid_contact_max, int row_count, int col_count, size_t* bytes);
+nb2_status launch_sensor_contact_update(const nb2_sensor_contact_view& sensor, const nb2_contacts_view& contacts, const float* body_q,
+                                        void* scratch, size_t scratch_bytes, cudaStream_t s);
 }  // namespace nb2
 
 #define NB2_CUDA_CHECK(expr)                                                                          \
