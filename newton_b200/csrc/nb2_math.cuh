@@ -108,6 +108,23 @@ NB2_DEV V3 qrot(Q4 q, V3 v) {
     return V3(v.x * c + q.x * d + (q.y * v.z - q.z * v.y) * w2, v.y * c + q.y * d + (q.z * v.x - q.x * v.z) * w2,
               v.z * c + q.z * d + (q.x * v.y - q.y * v.x) * w2);
 }
+// qrot(q, e_dim) for the basis vector e_dim (dim a compile-time constant after unrolling), with the products by the vector's 1 and 0
+// components left out.  Same remaining operations in the same order; the result differs from qrot's at most in the sign of an exact
+// zero component, so a caller must only use it where that sign cannot matter.
+NB2_DEV V3 qrot_basis(Q4 q, int dim) {
+    const float w2 = 2.0f * q.w;
+    const float c = w2 * q.w - 1.0f;
+    if (dim == 0) {
+        const float d = 2.0f * q.x;
+        return V3(c + q.x * d, q.y * d + q.z * w2, q.z * d - q.y * w2);
+    }
+    if (dim == 1) {
+        const float d = 2.0f * q.y;
+        return V3(q.x * d - q.z * w2, c + q.y * d, q.z * d + q.x * w2);
+    }
+    const float d = 2.0f * q.z;
+    return V3(q.x * d + q.y * w2, q.y * d - q.x * w2, c + q.z * d);
+}
 NB2_DEV V3 qrot_inv(Q4 q, V3 v) {
     const float w2 = 2.0f * q.w;
     float c = w2 * q.w - 1.0f;

@@ -85,38 +85,44 @@ NB2_HELPER float ang_inv_mass(const float* rec, V3 ang) {
     return dot(r, mv(ldm(rec + BR_INVI), r));
 }
 
-// shared denominators of compute_contact_constraint_delta / compute_positional_correction (kernels.py:2063-2075)
+// Exactness of the reduced expressions below.  Every value these helpers feed reaches the outputs either through a sum that starts
+// at +0.0f (the denominator here, the per-row delta accumulators, the per-body delta sums, the impulse accumulators) or through a
+// comparison; in round-to-nearest such a sum never holds -0 and is bit-identical whatever the signs of its zero addends.  So a
+// term that is an exact zero for finite operands (x * 0, a zero vector's len2) may be dropped from such a sum, and a reduced
+// expression that differs from the full one at most in the sign of an exact zero changes no output word, as long as that zero
+// cannot become a divisor.
+
+// shared denominators of compute_contact_constraint_delta / compute_positional_correction (kernels.py:2063-2075).  The static
+// world (rec == nullptr, inv_m = 0) adds len2(lin) * 0 = +0 to the sum: skipped.
 NB2_DEV float generalized_inv_mass(const BodyView& a, const BodyView& b, V3 lin_a, V3 lin_b, V3 ang_a, V3 ang_b) {
     float denom = 0.0f;
-    denom += len2(lin_a) * a.inv_m;
-    denom += len2(lin_b) * b.inv_m;
+    if (a.rec != nullptr) denom += len2(lin_a) * a.inv_m;
+    if (b.rec != nullptr) denom += len2(lin_b) * b.inv_m;
     denom += ang_inv_mass(a.rec, ang_a);
     denom += ang_inv_mass(b.rec, ang_b);
     return denom;
 }
-NB2_DEV float contact_delta(float err, const BodyView& a, const BodyView& b, V3 lin_a, V3 lin_b, V3 ang_a, V3 ang_b, float relaxation,
-                            float dt) {
-    float denom = generalized_inv_mass(a, b, lin_a, lin_b, ang_a, ang_b);
+// the same for a purely angular row (zero linear parts: len2(0) * inv_m = +0 for both bodies)
+NB2_DEV float angular_inv_mass(const BodyView& a, const BodyView& b, V3 ang_a, V3 ang_b) {
+    float denom = 0.0f;
+    denom += ang_inv_mass(a.rec, ang_a);
+    denom += ang_inv_mass(b.rec, ang_b);
+    return denom;
+}
+NB2_DEV float contact_delta(float err, float denom, float relaxation, float dt) {
     float dl = -err;
     if (denom > 0.0f) dl /= dt * denom;
     return dl * relaxation;
 }
-NB2_DEV float positional_correction(float err, float derr, const BodyView& a, const BodyView& b, V3 lin_a, V3 lin_b, V3 ang_a, V3 ang_b,
-                                    float compliance, float damping, float dt) {
-    float denom = generalized_inv_mass(a, b, lin_a, lin_b, ang_a, ang_b);
+// `param_alpha_dt` is the solver parameter's compliance / dt, formed once per substep; it replaces alpha / dt when `param` says
+// that alpha is that parameter.  The reference's `err + alpha * 0` term is dropped: alpha * 0 is +0 for a finite alpha, which can
+// only turn an err of -0 into +0, i.e. change the sign of a zero dl, and dl is a dividend whose products only enter the +0-started
+// delta sums.
+NB2_DEV float positional_correction(float err, float derr, float denom, float compliance, float damping, float dt, float param_alpha_dt,
+                                    bool param) {
     float alpha = compliance, gamma = compliance * damping;
-    float dl = -(err + alpha * 0.0f + gamma * derr);
-    if (denom + alpha > 0.0f) dl /= (dt + gamma) * denom + alpha / dt;
-    return dl;
-}
-NB2_DEV float angular_correction(float err, float derr, const BodyView& a, const BodyView& b, V3 ang_a, V3 ang_b, float compliance,
-                                 float damping, float dt) {
-    float denom = 0.0f;
-    denom += ang_inv_mass(a.rec, ang_a);
-    denom += ang_inv_mass(b.rec, ang_b);
-    float alpha = compliance, gamma = compliance * damping;
-    float dl = -(err + alpha * 0.0f + gamma * derr);
-    if (denom + alpha > 0.0f) dl /= (dt + gamma) * denom + alpha / dt;
+    float dl = -(err + gamma * derr);
+    if (denom + alpha > 0.0f) dl /= (dt + gamma) * denom + (param ? param_alpha_dt : alpha / dt);
     return dl;
 }
 
@@ -189,8 +195,9 @@ NB2_DEV AxisSetup load_axis_setup(const float* p) {
     return s;
 }
 
+// lin_alpha_dt / ang_alpha_dt: P.joint_linear_compliance / dt and P.joint_angular_compliance / dt, formed once per substep
 NB2_DEV bool solve_joint(const nb2_model_desc& d, const nb2_control_view& ctl, const nb2_xpbd_params& P, int j, int body0,
-                         const float* bodies, const float* jc, float dt, Deltas& out) {
+                         const float* bodies, const float* jc, float dt, float lin_alpha_dt, float ang_alpha_dt, Deltas& out) {
     // header: bits 0-3 type, bit 4 enabled, bits 8-11 / 12-15 linear / angular dof counts
     const int hdr = jc ? jc_int(jc, JC_HDR)
                        : (d.joint_type[j] | (d.joint_enabled[j] ? 16 : 0) | (d.joint_dof_dim[2 * j] << 8) | (d.joint_dof_dim[2 * j + 1] << 12));
@@ -247,7 +254,8 @@ NB2_DEV bool solve_joint(const nb2_model_desc& d, const nb2_control_view& ctl, c
             float ke = d.joint_target_ke[axis_start];
             if (ke > 0.0f) compliance = 1.0f / ke;
             float damping = d.joint_target_kd[axis_start];
-            float dl = positional_correction(err, derr, bp, bc, lp, lc, ap, ac, compliance, damping, dt);
+            float dl = positional_correction(err, derr, generalized_inv_mass(bp, bc, lp, lc, ap, ac), compliance, damping, dt, lin_alpha_dt,
+                                             !(ke > 0.0f));
             lin_dp += lp * (dl * P.joint_linear_relaxation);
             ang_dp += ap * (dl * P.joint_angular_relaxation);
             lin_dc += lc * (dl * P.joint_linear_relaxation);
@@ -268,11 +276,13 @@ NB2_DEV bool solve_joint(const nb2_model_desc& d, const nb2_control_view& ctl, c
         NB2_ROW_UNROLL
         for (int dim = 0; dim < 3; ++dim) {
             float e = rel_p.get(dim);
-            // column `dim` of quat_to_matrix(X_wp.q), i.e. the rotated basis vector
-            V3 lc = qrot(X_wp.q, V3(dim == 0 ? 1.f : 0.f, dim == 1 ? 1.f : 0.f, dim == 2 ? 1.f : 0.f));
+            // column `dim` of quat_to_matrix(X_wp.q), i.e. the rotated basis vector.  It differs from qrot(X_wp.q, e_dim) at most
+            // in the sign of a zero component; lc only enters products, |lc|^2 and +0-started sums (see the helpers above).
+            V3 lc = qrot_basis(X_wp.q, dim);
             V3 lp = -lc, ap = -cross(r_p, lc), ac = cross(r_c, lc);
             float derr = dot(lp, vel_p) + dot(lc, vel_c) + dot(ap, omega_p) + dot(ac, omega_c);
             float err = 0.0f, compliance = P.joint_linear_compliance, damping = 0.0f;
+            bool param = true;
             float derr_rel = derr - s.target_vel.get(dim);
             float lo = s.lim_lo.get(dim), up = s.lim_up.get(dim);
             if (e < lo) err = e - lo;
@@ -283,14 +293,17 @@ NB2_DEV bool solve_joint(const nb2_model_desc& d, const nb2_control_view& ctl, c
                 if (ks > 0.0f) {
                     err = e - tp;
                     compliance = 1.0f / ks;
+                    param = false;
                     damping = kdm;
                 } else if (kdm > 0.0f) {
                     compliance = 1.0f / kdm;
+                    param = false;
                     damping = kdm;
                 }
             }
             if (fabsf(err) > 1e-9f || fabsf(derr_rel) > 1e-9f) {
-                float dl = positional_correction(err, derr_rel, bp, bc, lp, lc, ap, ac, compliance, damping, dt);
+                float dl = positional_correction(err, derr_rel, generalized_inv_mass(bp, bc, lp, lc, ap, ac), compliance, damping, dt,
+                                                 lin_alpha_dt, param);
                 lin_dp += lp * (dl * P.joint_linear_relaxation);
                 ang_dp += ap * (dl * P.joint_angular_relaxation);
                 lin_dc += lc * (dl * P.joint_linear_relaxation);
@@ -304,21 +317,26 @@ NB2_DEV bool solve_joint(const nb2_model_desc& d, const nb2_control_view& ctl, c
         Q4 q_c = X_wc.q;
         if (qdot(q_p, q_c) < 0.0f) q_c = qscale(q_c, -1.0f);
         const Q4 rq = qmul(qconj(q_p), q_c);
-        const Q4 qtwist = qunit(Q4(rq.x, 0.0f, 0.0f, rq.w));
-        const Q4 qswing = qmul(rq, qconj(qtwist));
         const float sn = sqrtf(rq.x * rq.x + rq.w * rq.w);
         const float invs = 1.0f / sn;
         const float invscube = invs * invs * invs;
-        float err_0 = 2.0f * asin_w(clamp_w(qtwist.x, -1.0f, 1.0f));
-        float err_1 = qswing.y, err_2 = qswing.z;
-        Q4 g0(invs - rq.x * rq.x * invscube, 0.0f, 0.0f, -(rq.w * rq.x) * invscube);
+        // qtwist = qunit(Q4(rq.x, 0, 0, rq.w)).  Its squared norm (rq.x^2 + 0 * 0) + 0 * 0 + rq.w^2 is sn's argument bit for bit
+        // (rq.x^2 is never -0), so its length is sn and its scale invs.  Its y and z (+0) are not formed: qswing below leaves
+        // their terms out, which changes qswing at most by the sign of a zero (its y and z become the errors, its w enters
+        // squares, acos and a comparison)
+        const float tw_x = sn > 0.0f ? rq.x * invs : 0.0f, tw_w = sn > 0.0f ? rq.w * invs : 1.0f;
+        const float swing_y = tw_w * rq.y - rq.z * tw_x, swing_z = tw_w * rq.z + tw_x * rq.y, swing_w = rq.w * tw_w + rq.x * tw_x;
+        float err_0 = 2.0f * asin_w(clamp_w(tw_x, -1.0f, 1.0f));
+        float err_1 = swing_y, err_2 = swing_z;
+        // the twist gradient (x, 0, 0, w) scaled by 2 / |qtwist.w|: its y and z stay zero, so only x and w are formed
+        const float g0_scale = 2.0f / fabsf(tw_w);
+        const float g0x = (invs - rq.x * rq.x * invscube) * g0_scale, g0w = (-(rq.w * rq.x) * invscube) * g0_scale;
         Q4 g1(-rq.w * (rq.w * rq.z + rq.x * rq.y) * invscube, rq.w * invs, -rq.x * invs, rq.x * (rq.w * rq.z + rq.x * rq.y) * invscube);
         Q4 g2(rq.w * (rq.w * rq.y - rq.x * rq.z) * invscube, rq.x * invs, rq.w * invs, rq.x * (rq.z * rq.x - rq.w * rq.y) * invscube);
-        g0 = qscale(g0, 2.0f / fabsf(qtwist.w));
-        const float swing_sq = qswing.w * qswing.w;
+        const float swing_sq = swing_w * swing_w;
         if (swing_sq + 1.0e-4f < 1.0f) {
-            float dd = sqrtf(1.0f - qswing.w * qswing.w);
-            float theta = 2.0f * acos_w(clamp_w(qswing.w, -1.0f, 1.0f));
+            float dd = sqrtf(1.0f - swing_w * swing_w);
+            float theta = 2.0f * acos_w(clamp_w(swing_w, -1.0f, 1.0f));
             float scale = theta / dd;
             err_1 *= scale;
             err_2 *= scale;
@@ -327,16 +345,24 @@ NB2_DEV bool solve_joint(const nb2_model_desc& d, const nb2_control_view& ctl, c
         }
         const AxisSetup s = jc ? load_axis_setup(jc + JC_ANG) : gather_axes(d, ctl, axis_start, target_start, lin_count, ang_count);
         const Q4 qc_inv = qconj(q_c);
+        const Q4 hp = qscale(q_p, 0.5f);
         NB2_ROW_UNROLL
         for (int dim = 0; dim < 3; ++dim) {
             float e = dim == 0 ? err_0 : (dim == 1 ? err_1 : err_2);
-            Q4 grad = dim == 0 ? g0 : (dim == 1 ? g1 : g2);
-            Q4 quat_c = qmul(qmul(qscale(q_p, 0.5f), grad), qc_inv);
+            // qmul(hp, g0) without the terms of g0's zero y and z: the result differs at most in the sign of a zero component,
+            // and ac / ap only enter products, |ac| and +0-started sums
+            Q4 hg = dim == 0 ? Q4(hp.w * g0x + g0w * hp.x, g0w * hp.y + hp.z * g0x, g0w * hp.z - g0x * hp.y, hp.w * g0w - hp.x * g0x)
+                             : qmul(hp, dim == 1 ? g1 : g2);
+            Q4 quat_c = qmul(hg, qc_inv);
             V3 ac(quat_c.x, quat_c.y, quat_c.z);
             V3 ap = -ac;
             float derr = dot(ap, omega_p) + dot(ac, omega_c);
             float err = 0.0f, compliance = P.joint_angular_compliance, damping = 0.0f;
-            float derr_rel = derr - s.target_vel.get(dim) * len(ac);
+            bool param = true;
+            // target_vel is a +0-started sum (over a positive damping), never -0: when it is zero the reference subtracts
+            // +0 * |ac| = +0 (finite ac), and derr - (+0) == derr for every derr
+            const float tv = s.target_vel.get(dim);
+            float derr_rel = tv == 0.0f ? derr : derr - tv * len(ac);
             float lo = s.lim_lo.get(dim), up = s.lim_up.get(dim);
             if (e < lo) err = e - lo;
             else if (e > up) err = e - up;
@@ -346,13 +372,16 @@ NB2_DEV bool solve_joint(const nb2_model_desc& d, const nb2_control_view& ctl, c
                 if (ks > 0.0f) {
                     err = e - tp;
                     compliance = 1.0f / ks;
+                    param = false;
                     damping = kdm;
                 } else if (kdm > 0.0f) {
                     damping = kdm;
                     compliance = 1.0f / kdm;
+                    param = false;
                 }
             }
-            float dl = angular_correction(err, derr_rel, bp, bc, ap, ac, compliance, damping, dt) * P.joint_angular_relaxation;
+            float dl = positional_correction(err, derr_rel, angular_inv_mass(bp, bc, ap, ac), compliance, damping, dt, ang_alpha_dt, param) *
+                       P.joint_angular_relaxation;
             ang_dp += ap * dl;
             ang_dc += ac * dl;
         }
@@ -440,15 +469,22 @@ NB2_HELPER void apply_delta(float* rec, V3 dlin, V3 dang, float inv_weight, bool
     const V3 tb = cross(dwb, mv(I, wb + dwb)) + cross(wb, mv(I, dwb));
     const V3 dw1 = qrot(q0, dwb - mv(mscale(dt, inv_I), tb));
     const V3 h = dw1 * dt;
-    Q4 q1 = qadd(q0, qmul(qscale(Q4(h.x, h.y, h.z, 0.0f), 0.5f), q0));
+    // q0 + qmul((0.5 h, 0), q0) without qmul's leading products of the zero w, (+0) * q0.c.  That term has the sign of q0.c: when
+    // q0.c is negative it is -0, an exact identity of the sum; otherwise it can only turn a zero sum into +0, and q0.c + (+-0) with
+    // q0.c >= +0 is q0.c either way.  So q1 is bit-identical.
+    const V3 hh = h * 0.5f;
+    Q4 q1 = qadd(q0, Q4(q0.w * hh.x + hh.y * q0.z - q0.y * hh.z, q0.w * hh.y + hh.z * q0.x - q0.z * hh.x,
+                        q0.w * hh.z + hh.x * q0.y - q0.x * hh.y, -hh.x * q0.x - hh.y * q0.y - hh.z * q0.z));
     q1 = qunit(q1);
     const V3 com = ld3(rec + BR_COM);
     const V3 x_com = p0 + qrot(q0, com);
     V3 p1 = x_com + dp * dt;
     p1 -= qrot(q1, com);
     V3 v1 = v0 + dp, w1 = w0 + dw1;
-    if (len(v1) < 1e-4f) v1 = V3();
-    if (len(w1) < 1e-4f) w1 = V3();
+    // len(v) < 1e-4f without the square root: sqrtf is correctly rounded and monotonic, and 0x1.5798ecp-27f (1e-4f * 1e-4f rounded)
+    // is the smallest float whose square root rounds to 1e-4f or more, so the two tests agree for every input, NaN included
+    if (len2(v1) < 0x1.5798ecp-27f) v1 = V3();
+    if (len2(w1) < 0x1.5798ecp-27f) w1 = V3();
     st3(rec + BR_Q, p1);
     rec[BR_Q + 3] = q1.x; rec[BR_Q + 4] = q1.y; rec[BR_Q + 5] = q1.z; rec[BR_Q + 6] = q1.w;
     st3(rec + BR_QD, v1);
@@ -738,6 +774,7 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
     // ---- Jacobi iterations ---------------------------------------------------------------------------
     const size_t T = size_t(M.slot_total);
     const float* cb = M.cb;
+    const float lin_alpha_dt = P.joint_linear_compliance / dt, ang_alpha_dt = P.joint_angular_compliance / dt;
     for (int it = 0; it < P.iterations; ++it) {
         // CTA barriers are not needed for correctness (a warp owns its environments); they keep the CTA's warps on the same
         // stretch of code so that the instruction stream is fetched once per CTA (see the kernel comment)
@@ -762,7 +799,9 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
                     const V3 p0 = cached ? ld3(cc + CC_P0) : V3(cb[CF_P0X * T + s], cb[CF_P0Y * T + s], cb[CF_P0Z * T + s]);
                     const V3 p1 = cached ? ld3(cc + CC_P1) : V3(cb[CF_P1X * T + s], cb[CF_P1Y * T + s], cb[CF_P1Z * T + s]);
                     const V3 n = cached ? ld3(cc + CC_N) : V3(cb[CF_NX * T + s], cb[CF_NY * T + s], cb[CF_NZ * T + s]);
-                    V3 bx_a = ba >= 0 ? xpoint(A.X, p0) : V3() + p0, bx_b = bb >= 0 ? xpoint(B.X, p1) : V3() + p1;
+                    // static side: p instead of the reference's (+0) + p, which differ at most in the sign of a zero
+                    // coordinate; bx only enters differences, products and |fd|, a comparison and +0-started sums
+                    V3 bx_a = ba >= 0 ? xpoint(A.X, p0) : p0, bx_b = bb >= 0 ? xpoint(B.X, p1) : p1;
                     const float dpen = dot(n, bx_b - bx_a) - (cached ? cc[CC_MSUM] : cb[CF_MARGIN0 * T + s] + cb[CF_MARGIN1 * T + s]);
                     if (dpen < 0.0f) {
                         active = 1.0f;
@@ -773,7 +812,7 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
                         V3 ang_a, ang_b;
                         if (need_a) ang_a = -cross(r_a, n);
                         if (need_b) ang_b = cross(r_b, n);
-                        const float lambda_n = contact_delta(dpen, A, B, -n, n, ang_a, ang_b, P.rigid_contact_relaxation, dt);
+                        const float lambda_n = contact_delta(dpen, generalized_inv_mass(A, B, -n, n, ang_a, ang_b), P.rigid_contact_relaxation, dt);
                         V3 lin_da, lin_db, ang_da, ang_db;
                         if (need_a) { lin_da = -n * lambda_n; ang_da = ang_a * lambda_n; }
                         if (need_b) { lin_db = n * lambda_n; ang_db = ang_b * lambda_n; }
@@ -786,8 +825,8 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
                                 q0 = p0 + V3(cb[CF_O0X * T + s], cb[CF_O0Y * T + s], cb[CF_O0Z * T + s]);
                                 q1 = p1 + V3(cb[CF_O1X * T + s], cb[CF_O1Y * T + s], cb[CF_O1Z * T + s]);
                             }
-                            bx_a = ba >= 0 ? xpoint(A.X, q0) : V3() + q0;
-                            bx_b = bb >= 0 ? xpoint(B.X, q1) : V3() + q1;
+                            bx_a = ba >= 0 ? xpoint(A.X, q0) : q0;  // static side as above
+                            bx_b = bb >= 0 ? xpoint(B.X, q1) : q1;
                             V3 delta = bx_b - bx_a;
                             V3 fd = delta - dot(n, delta) * n;
                             r_a = bx_a - wcom_a;
@@ -807,7 +846,8 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
                             if (need_b) ang_b = cross(r_b, perp);
                             float err = len(fd);
                             if (err > 0.0f) {
-                                float lambda_fr = contact_delta(err, A, B, -perp, perp, ang_a, ang_b, P.rigid_contact_relaxation, dt);
+                                float lambda_fr =
+                                    contact_delta(err, generalized_inv_mass(A, B, -perp, perp, ang_a, ang_b), P.rigid_contact_relaxation, dt);
                                 lambda_fr = fmax_w(lambda_fr, -lambda_n * mu);
                                 if (need_a) { lin_da -= perp * lambda_fr; ang_da += ang_a * lambda_fr; }
                                 if (need_b) { lin_db += perp * lambda_fr; ang_db += ang_b * lambda_fr; }
@@ -817,7 +857,7 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
                         if (mu_t > 0.0f) {
                             float err = dot(dom, n) * dt;
                             if (fabsf(err) > 0.0f) {
-                                float lt = contact_delta(err, A, B, V3(), V3(), -n, n, P.rigid_contact_relaxation, dt);
+                                float lt = contact_delta(err, angular_inv_mass(A, B, -n, n), P.rigid_contact_relaxation, dt);
                                 lt = clamp_w(lt, -lambda_n * mu_t, lambda_n * mu_t);
                                 if (need_a) ang_da -= n * lt;
                                 if (need_b) ang_db += n * lt;
@@ -828,7 +868,7 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
                             float err = len(dom) * dt;
                             if (err > 0.0f) {
                                 V3 rn = unit(dom);
-                                float lr = contact_delta(err, A, B, V3(), V3(), -rn, rn, P.rigid_contact_relaxation, dt);
+                                float lr = contact_delta(err, angular_inv_mass(A, B, -rn, rn), P.rigid_contact_relaxation, dt);
                                 lr = fmax_w(lr, -lambda_n * mu_r);
                                 if (need_a) ang_da -= rn * lr;
                                 if (need_b) ang_db += rn * lr;
@@ -901,7 +941,8 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
             // ---- [iteration] solve_body_joints (kernels.py:1513-2044) + ordered per-body apply
             for (int j = l; j < nj; j += L) {
                 Deltas dl;
-                bool act = solve_joint(d, ctl, P, j0 + j, b0, bodies, jcache ? jcache + j * JC_SIZE : nullptr, dt, dl);
+                bool act = solve_joint(d, ctl, P, j0 + j, b0, bodies, jcache ? jcache + j * JC_SIZE : nullptr, dt, lin_alpha_dt,
+                                       ang_alpha_dt, dl);
                 if (!act) dl = Deltas();
                 store_deltas(drec + j * DR_SIZE, dl, act ? 1.0f : 0.0f);
                 if (want_jimp && act) {  // kernels.py:2043-2044
