@@ -488,6 +488,85 @@ nb2_status nb2_intersect_ray(const nb2_raycast_view* view, int32_t ray_count, co
                              const int32_t* ray_worlds, int32_t enable_global_world, float* out_dist, int32_t* out_shape_id,
                              float* out_normal, void* cuda_stream);
 
+/* --- actuators (reference newton.actuators, actuators/) --------------------------------------------------------------------
+ * One thread per actuator of one group: delayed or current targets -> PD / PID -> clamp chain -> out[idx] = out[idx] + f ->
+ * delay buffer and PID state of the next state.  Index arrays are int32 (the reference's uint32 values).  The host
+ * (newton_b200.actuators.Actuator) fills the descriptor; the library keeps no per-actuator state, allocates nothing and does
+ * not synchronise, so a step can be captured into a CUDA graph.  Strict fp32 in the reference's operation order. */
+enum { NB2_ACT_PD = 0, NB2_ACT_PID = 1 };
+enum { NB2_CLAMP_MAX_EFFORT = 1, NB2_CLAMP_DC_MOTOR = 2, NB2_CLAMP_POSITION_BASED = 3 };
+enum { NB2_ACTUATOR_MAX_CLAMPS = 8, NB2_ACTUATOR_MAX_LOOKUP = 2048 };
+
+typedef struct nb2_actuator_clamp {
+    int32_t kind;          /* NB2_CLAMP_* */
+    int32_t lookup_size;   /* POSITION_BASED: table length (the table is shared by the group) */
+    const float* p0;       /* MAX_EFFORT: max_effort [N]; DC_MOTOR: saturation_effort [N]; POSITION_BASED: positions [K] */
+    const float* p1;       /* DC_MOTOR: velocity_limit [N]; POSITION_BASED: efforts [K] */
+    const float* p2;       /* DC_MOTOR: max_motor_effort [N] */
+} nb2_actuator_clamp;
+
+typedef struct nb2_actuator_step_desc {
+    int32_t count;              /* N actuators */
+    int32_t controller;         /* NB2_ACT_PD / NB2_ACT_PID */
+    int32_t clamp_count;        /* <= NB2_ACTUATOR_MAX_CLAMPS, applied in order */
+    int32_t buf_depth;          /* delay buffer depth (max_delay); 0 = no delay */
+    float dt;                   /* PID only */
+    const int32_t* indices;             /* [N] dof layout: velocities, target velocities, feedforward */
+    const int32_t* pos_indices;         /* [N] coordinate layout: positions */
+    const int32_t* target_pos_indices;  /* [N] into target_pos */
+    const int32_t* effort_indices;      /* [N] into output / computed_output */
+    const float* positions;
+    const float* velocities;
+    const float* target_pos;
+    const float* target_vel;
+    const float* feedforward;    /* may be NULL (reads as 0) */
+    const float* kp;
+    const float* ki;             /* PID */
+    const float* kd;
+    const float* integral_max;   /* PID */
+    const float* const_effort;   /* may be NULL (reads as 0) */
+    const float* integral_in;    /* PID: current state */
+    float* integral_out;         /* PID: next state */
+    const int32_t* delay_steps;  /* [N] when buf_depth > 0; the delay buffers are [buf_depth, N] */
+    const float* buf_pos_in;
+    const float* buf_vel_in;
+    const float* buf_act_in;
+    const int32_t* num_pushes_in;
+    const int32_t* write_idx_in; /* [1] */
+    float* buf_pos_out;
+    float* buf_vel_out;
+    float* buf_act_out;
+    int32_t* num_pushes_out;
+    int32_t* write_idx_out;      /* [1]: distinct storage from write_idx_in */
+    float* output;               /* applied effort, accumulated */
+    float* computed_output;      /* pre-clamp effort, accumulated; may be NULL */
+    /* Duplicate effort indices: when dup_target_count > 0 the efforts go to scratch ([2N]: applied, computed) and a second
+     * launch adds them per distinct target in ascending actuator index (dup_start[T + 1] CSR over dup_actuator[N]). */
+    int32_t dup_target_count;
+    const int32_t* dup_target;
+    const int32_t* dup_start;
+    const int32_t* dup_actuator;
+    float* scratch;
+    nb2_actuator_clamp clamps[NB2_ACTUATOR_MAX_CLAMPS];
+} nb2_actuator_step_desc;
+
+/* Reference Actuator.step (actuators/actuator.py:204-332) for one group. */
+nb2_status nb2_actuator_step(const nb2_actuator_step_desc* desc, void* cuda_stream);
+
+/* Reference Delay.State.reset / ControllerPID.State.reset: mask NULL = full reset (buffers, num_pushes and integral zeroed,
+ * write_idx = buf_depth - 1); otherwise the masked columns are zeroed and write_idx is left alone.  Any of the state pointers
+ * may be NULL (buf_depth 0 for no delay state). */
+nb2_status nb2_actuator_reset(int32_t count, int32_t buf_depth, const uint8_t* mask, float* buf_pos, float* buf_vel, float* buf_act,
+                              int32_t* num_pushes, int32_t* write_idx, float* integral, void* cuda_stream);
+
+/* ArticulationView actuator parameters: `map` [world_count * dofs_per_world] holds the parameter index of each view dof, or -1.
+ * gather writes values[k] = map[k] >= 0 ? param[map[k]] : 0; scatter writes param[map[k]] = values[k] for mapped entries of
+ * the worlds whose world_mask entry is set (NULL = all).  `is_int`: the parameter and values are int32, else float32. */
+nb2_status nb2_actuator_param_gather(const int32_t* map, int32_t entries, const void* param, void* values, int32_t is_int,
+                                     void* cuda_stream);
+nb2_status nb2_actuator_param_scatter(const int32_t* map, int32_t entries, int32_t dofs_per_world, const uint8_t* world_mask,
+                                      const void* values, void* param, int32_t is_int, void* cuda_stream);
+
 /* --- multi-GPU end-of-frame state gather without compute kernels (SURVEY.md §8(e)) --------------------------------------
  * Replaces the `ncclAllGather(body_q, body_qd)` of the reference design (there is no reference code for it: upstream is
  * single-GPU; the sharding follows sim/model.py:1081-1097 world ranges).  Every rank owns a receive buffer of

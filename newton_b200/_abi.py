@@ -238,6 +238,30 @@ class RaycastView(C.Structure):
 RAYCAST_MAX_DEPTH = 48  # NB2_RAYCAST_MAX_DEPTH
 
 
+ACT_PD, ACT_PID = 0, 1  # NB2_ACT_*
+CLAMP_MAX_EFFORT, CLAMP_DC_MOTOR, CLAMP_POSITION_BASED = 1, 2, 3  # NB2_CLAMP_*
+ACTUATOR_MAX_CLAMPS, ACTUATOR_MAX_LOOKUP = 8, 2048  # NB2_ACTUATOR_MAX_*
+
+
+class ActuatorClamp(C.Structure):
+    """``nb2_actuator_clamp``"""
+
+    _fields_ = [("kind", C.c_int32), ("lookup_size", C.c_int32), ("p0", C.c_void_p), ("p1", C.c_void_p), ("p2", C.c_void_p)]
+
+
+class ActuatorStepDesc(C.Structure):
+    """``nb2_actuator_step_desc``"""
+
+    _fields_ = [("count", C.c_int32), ("controller", C.c_int32), ("clamp_count", C.c_int32), ("buf_depth", C.c_int32),
+                ("dt", C.c_float)] + [(n, C.c_void_p) for n in (
+                    "indices", "pos_indices", "target_pos_indices", "effort_indices", "positions", "velocities", "target_pos",
+                    "target_vel", "feedforward", "kp", "ki", "kd", "integral_max", "const_effort", "integral_in", "integral_out",
+                    "delay_steps", "buf_pos_in", "buf_vel_in", "buf_act_in", "num_pushes_in", "write_idx_in", "buf_pos_out",
+                    "buf_vel_out", "buf_act_out", "num_pushes_out", "write_idx_out", "output", "computed_output")] + [
+                ("dup_target_count", C.c_int32), ("dup_target", C.c_void_p), ("dup_start", C.c_void_p), ("dup_actuator", C.c_void_p),
+                ("scratch", C.c_void_p), ("clamps", ActuatorClamp * ACTUATOR_MAX_CLAMPS)]
+
+
 class FeatherstoneParams(C.Structure):
     _fields_ = [
         ("angular_damping", C.c_float),

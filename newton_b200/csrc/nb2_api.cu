@@ -1009,6 +1009,93 @@ nb2_status nb2_intersect_ray(const nb2_raycast_view* view, int32_t ray_count, co
                                 out_normal, static_cast<cudaStream_t>(cuda_stream));
 }
 
+nb2_status nb2_actuator_step(const nb2_actuator_step_desc* desc, void* cuda_stream) {
+    if (!desc) {
+        set_error("nb2_actuator_step: NULL descriptor");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    const nb2_actuator_step_desc& d = *desc;
+    if (d.count < 0 || d.buf_depth < 0 || d.clamp_count < 0 || d.dup_target_count < 0 ||
+        (d.controller != NB2_ACT_PD && d.controller != NB2_ACT_PID)) {
+        set_error("nb2_actuator_step: invalid count, buf_depth, clamp_count or controller");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    if (d.clamp_count > NB2_ACTUATOR_MAX_CLAMPS) {
+        set_error("nb2_actuator_step: a clamp chain holds at most " + std::to_string(NB2_ACTUATOR_MAX_CLAMPS) + " clampings, got " +
+                  std::to_string(d.clamp_count));
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    if (d.count == 0) return NB2_OK;
+    if (!d.indices || !d.pos_indices || !d.target_pos_indices || !d.effort_indices || !d.positions || !d.velocities || !d.target_pos ||
+        !d.target_vel || !d.kp || !d.kd || !d.output) {
+        set_error("nb2_actuator_step: NULL index, state, control, gain or output array");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    if (d.controller == NB2_ACT_PID && (!d.ki || !d.integral_max || !d.integral_in || !d.integral_out)) {
+        set_error("nb2_actuator_step: PID needs ki, integral_max and the integral of both states");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    if (d.buf_depth > 0 && (!d.delay_steps || !d.buf_pos_in || !d.buf_vel_in || !d.buf_act_in || !d.num_pushes_in || !d.write_idx_in ||
+                            !d.buf_pos_out || !d.buf_vel_out || !d.buf_act_out || !d.num_pushes_out || !d.write_idx_out)) {
+        set_error("nb2_actuator_step: a delay needs delay_steps and the buffers of both states");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    if (d.buf_depth > 0 && d.write_idx_in == d.write_idx_out) {
+        set_error("nb2_actuator_step: the current and next delay states share write_idx storage");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    if (d.dup_target_count > 0 && (!d.dup_target || !d.dup_start || !d.dup_actuator || !d.scratch)) {
+        set_error("nb2_actuator_step: duplicate effort indices need the per-target lists and scratch");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    int lookup = 0;
+    for (int c = 0; c < d.clamp_count; ++c) {
+        const nb2_actuator_clamp& k = d.clamps[c];
+        const bool ok = (k.kind == NB2_CLAMP_MAX_EFFORT && k.p0) || (k.kind == NB2_CLAMP_DC_MOTOR && k.p0 && k.p1 && k.p2) ||
+                        (k.kind == NB2_CLAMP_POSITION_BASED && k.lookup_size > 0 && k.p0 && k.p1);
+        if (!ok) {
+            set_error("nb2_actuator_step: clamp " + std::to_string(c) + " has an unknown kind or NULL parameters");
+            return NB2_ERR_INVALID_ARGUMENT;
+        }
+        if (k.kind == NB2_CLAMP_POSITION_BASED) lookup += k.lookup_size;
+    }
+    if (lookup > NB2_ACTUATOR_MAX_LOOKUP) {
+        set_error("nb2_actuator_step: the lookup tables of one group hold at most " + std::to_string(NB2_ACTUATOR_MAX_LOOKUP) +
+                  " entries, got " + std::to_string(lookup));
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    return launch_actuator_step(d, static_cast<cudaStream_t>(cuda_stream));
+}
+
+nb2_status nb2_actuator_reset(int32_t count, int32_t buf_depth, const uint8_t* mask, float* buf_pos, float* buf_vel, float* buf_act,
+                              int32_t* num_pushes, int32_t* write_idx, float* integral, void* cuda_stream) {
+    if (count < 0 || buf_depth < 0 || (buf_pos && (!buf_vel || !buf_act || buf_depth == 0))) {
+        set_error("nb2_actuator_reset: invalid count, buf_depth or buffers");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    return launch_actuator_reset(count, buf_depth, mask, buf_pos, buf_vel, buf_act, num_pushes, write_idx, integral,
+                                 static_cast<cudaStream_t>(cuda_stream));
+}
+
+nb2_status nb2_actuator_param_gather(const int32_t* map, int32_t entries, const void* param, void* values, int32_t is_int,
+                                     void* cuda_stream) {
+    if (entries < 0 || (entries > 0 && (!map || !param || !values))) {
+        set_error("nb2_actuator_param_gather: invalid entries or NULL array");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    return launch_actuator_param(true, map, entries, 1, nullptr, param, values, is_int != 0, static_cast<cudaStream_t>(cuda_stream));
+}
+
+nb2_status nb2_actuator_param_scatter(const int32_t* map, int32_t entries, int32_t dofs_per_world, const uint8_t* world_mask,
+                                      const void* values, void* param, int32_t is_int, void* cuda_stream) {
+    if (entries < 0 || dofs_per_world <= 0 || (entries > 0 && (!map || !param || !values))) {
+        set_error("nb2_actuator_param_scatter: invalid entries, dofs_per_world or NULL array");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    return launch_actuator_param(false, map, entries, dofs_per_world, world_mask, values, param, is_int != 0,
+                                 static_cast<cudaStream_t>(cuda_stream));
+}
+
 const char* nb2_last_error(void) { return g_last_error.c_str(); }
 int64_t nb2_kernel_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
 const char* nb2_version(void) { return "newton_b200 0.1 (sm_90a)"; }

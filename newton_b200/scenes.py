@@ -21,6 +21,7 @@ import torch
 
 from .utils.host_fk import host_fk  # noqa: F401  (re-exported: scenes.host_fk)
 from .sim.builder import ModelBuilder, ShapeConfig
+from .sim.enums import JointType
 from .utils import xform as X
 
 _HALF_PI = "1.57079632679"
@@ -96,6 +97,39 @@ def quadruped_model(world_count: int, device="cpu", seed: int | None = 1, noise:
     targets follow; ``seed=None`` keeps every env identical to the stock example.
     """
     quad = quadruped_builder()
+    scene = ModelBuilder()
+    scene.replicate(quad, world_count)
+    scene.add_ground_plane(cfg=quad.default_shape_cfg)
+    if seed is not None and noise > 0.0:
+        rng = np.random.default_rng(seed)
+        per = quad.joint_coord_count
+        jq = np.asarray(scene.joint_q, dtype=np.float64).reshape(world_count, per)
+        jq[:, 7:] += rng.normal(0.0, noise, size=(world_count, per - 7))
+        scene.joint_q = jq.reshape(-1).tolist()
+        scene.joint_target_q = list(scene.joint_q)
+    return _finish(scene, device)
+
+
+def quadruped_actuated_model(world_count: int, device="cpu", seed: int | None = 1, noise: float = 0.02, controller: str = "pd"):
+    """:func:`quadruped_model` driven through actuators: the 12 leg dofs of every quadruped form one group of PD (or PID with
+    ``controller="pid"``) + ``ClampingDCMotor`` + ``Delay`` with delays of 1, 2 and 3 steps in turn.  The controller gains
+    are the stock drive gains (kp 2000, kd 1), and the model's own ``joint_target_ke / kd`` are zeroed so that the
+    solver's built-in drive adds nothing."""
+    from .actuators import ClampingDCMotor, ControllerPD, ControllerPID
+
+    quad = quadruped_builder()
+    legs = [j for j in range(quad.joint_count) if quad.joint_type[j] == JointType.REVOLUTE]
+    dc = {"saturation_effort": 120.0, "velocity_limit": 30.0, "max_motor_effort": 80.0}
+    for k, j in enumerate(legs):
+        dof, coord = quad.joint_qd_start[j], quad.joint_q_start[j]
+        gains = {"kp": quad.joint_target_ke[dof], "kd": quad.joint_target_kd[dof]}
+        if controller == "pid":
+            quad.add_actuator(ControllerPID, index=dof, pos_index=coord, delay_steps=1 + k % 3, clamping=[(ClampingDCMotor, dc)],
+                              ki=10.0, integral_max=0.1, **gains)
+        else:
+            quad.add_actuator(ControllerPD, index=dof, pos_index=coord, delay_steps=1 + k % 3, clamping=[(ClampingDCMotor, dc)], **gains)
+        quad.joint_target_ke[dof] = 0.0
+        quad.joint_target_kd[dof] = 0.0
     scene = ModelBuilder()
     scene.replicate(quad, world_count)
     scene.add_ground_plane(cfg=quad.default_shape_cfg)

@@ -592,3 +592,76 @@ class ArticulationView:
 
         eval_inverse_dynamics_force(self.model, state, mass_matrix=mass_matrix, joint_qdd=joint_qdd, coriolis_force=coriolis_force,
                                     gravity_force=gravity_force, joint_f=joint_f, mask=self.get_model_articulation_mask(mask=mask))
+
+    # ------------------------------------------------------------------ actuator parameters (selection.py:1923-2100)
+    def _actuator_dof_mapping(self, actuator):
+        """``[world_count * dofs_per_world]`` int32: the parameter index of ``actuator`` driving each view dof, or -1.  Built on
+        the host the first time it is asked for, then cached per actuator.  A dof driven by several of the actuator's entries
+        maps to the lowest of them."""
+        cache = self.__dict__.setdefault("_actuator_maps", {})
+        hit = cache.get(id(actuator))
+        if hit is not None and hit[0] is actuator:
+            return hit[1]
+        layout = self.frequency_layouts[AttributeFrequency.JOINT_DOF]
+        per_arti = layout.selected_value_count
+        sel = (np.arange(layout.slice.start, layout.slice.stop) if layout.is_contiguous else layout.indices.cpu().numpy()).astype(np.int64)
+        w = np.arange(self.world_count, dtype=np.int64)[:, None, None]
+        a = np.arange(self.count_per_world, dtype=np.int64)[None, :, None]
+        dofs = (layout.offset + w * layout.stride_between_worlds + a * layout.stride_within_worlds + sel[None, None, :]).reshape(-1)
+        first = {}
+        for j, d in enumerate(actuator.indices.cpu().numpy().tolist()):
+            first.setdefault(d, j)
+        mapping = np.array([first.get(int(d), -1) for d in dofs], dtype=np.int32)
+        out = torch.from_numpy(mapping).to(self.device)
+        cache[id(actuator)] = (actuator, out)
+        return out
+
+    @staticmethod
+    def _actuator_param_kind(param, name):
+        if param.dtype == torch.float32:
+            return 0
+        if param.dtype == torch.int32:
+            return 1
+        raise TypeError(f"actuator parameter '{name}' has dtype {param.dtype}; float32 and int32 parameters are supported")
+
+    def get_actuator_parameter(self, actuator, component, name: str):
+        """``component.<name>`` for every dof of the view, shaped ``(world_count, dofs_per_world)``; dofs ``actuator`` does not
+        drive read 0.  One launch; can be captured in a CUDA graph once the mapping is cached."""
+        from .actuators.actuator import _call
+
+        mapping = self._actuator_dof_mapping(actuator)
+        src = getattr(component, name)
+        is_int = self._actuator_param_kind(src, name)
+        dst = torch.empty(mapping.numel(), dtype=src.dtype, device=self.device)
+        if mapping.numel():
+            _call("param_gather", self.device, _abi.ptr(mapping, "i32", self.device, None, "mapping"), int(mapping.numel()),
+                  _abi.ptr(src, "i32" if is_int else "f32", self.device, actuator.num_actuators, name),
+                  dst.data_ptr(), is_int)
+        return dst.reshape(self.world_count, -1)
+
+    def set_actuator_parameter(self, actuator, component, name: str, values, mask=None) -> None:
+        """Write ``values`` ``(world_count, dofs_per_world)`` into ``component.<name>`` for the dofs ``actuator`` drives, in the
+        worlds where the per-world ``mask`` is set (all by default); the other entries are ignored.  The mask and values are
+        checked before the launch."""
+        from .actuators.actuator import _call
+
+        world_mask = self._resolve_world_mask(mask)
+        mapping = self._actuator_dof_mapping(actuator)
+        dst = getattr(component, name)
+        is_int = self._actuator_param_kind(dst, name)
+        dpw = mapping.numel() // self.world_count if self.world_count else 0
+        if not isinstance(values, torch.Tensor):
+            values = torch.as_tensor(np.asarray(values), dtype=dst.dtype).to(self.device)
+        if tuple(values.shape) != (self.world_count, dpw):
+            raise ValueError(f"Expected values with shape ({self.world_count}, {dpw}), got {tuple(values.shape)}")
+        if values.dtype != dst.dtype:
+            raise ValueError(f"Expected values of dtype {dst.dtype}, got {values.dtype}")
+        if not _same_device(values.device, self.device):
+            raise ValueError(f"Expected values on device {self.device}, got {values.device}")
+        if mapping.numel() == 0:
+            return
+        kind = "i32" if is_int else "f32"
+        values = values.contiguous()
+        _call("param_scatter", self.device, _abi.ptr(mapping, "i32", self.device, None, "mapping"), int(mapping.numel()), dpw,
+              _abi.ptr(world_mask, "bool", self.device, self.world_count, "mask"), _abi.ptr(values, kind, self.device, None, "values"),
+              _abi.ptr(dst, kind, self.device, actuator.num_actuators, name), is_int)

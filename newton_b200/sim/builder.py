@@ -24,8 +24,10 @@ from __future__ import annotations
 
 import copy
 import math
+import warnings
 import xml.etree.ElementTree as ET
-from dataclasses import dataclass
+from dataclasses import dataclass, field
+from typing import Any
 
 import numpy as np
 import torch
@@ -144,11 +146,41 @@ _FINALIZE_SHAPE = ("shape_collision_aabb_lower", "shape_collision_aabb_upper", "
 _PER_SHAPE = [n for n in _SHAPE_FIELDS if n not in _FINALIZE_SHAPE]
 
 
+@dataclass
+class ActuatorEntry:
+    """One group of compatible actuators accumulated by :meth:`ModelBuilder.add_actuator` (reference
+    ``ModelBuilder.ActuatorEntry``): the controller class, the clamping classes with their shared (per-group) arguments and
+    the controller's shared arguments are the same for every member; the rest is per actuator."""
+
+    controller_class: type
+    clamping_classes: tuple
+    clamping_shared_kwargs: tuple
+    controller_shared_kwargs: dict
+    indices: list = field(default_factory=list)  # dof indices (joint_qd layout)
+    pos_indices: list = field(default_factory=list)  # coordinate indices (joint_q layout)
+    controller_args: list = field(default_factory=list)
+    delay_args: list = field(default_factory=list)  # empty when the group has no delay
+    clamping_args: list = field(default_factory=list)  # per actuator: one dict per clamping
+
+
+def _split_shared(component_class, resolved: dict) -> tuple[dict, dict]:
+    """``resolved`` arguments of an actuator component as (shared by its whole group, per actuator)."""
+    shared_names = getattr(component_class, "SHARED_PARAMS", ())
+    group = {k: v for k, v in resolved.items() if k in shared_names}
+    return group, {k: v for k, v in resolved.items() if k not in group}
+
+
+def _frozen(args: dict) -> tuple:
+    """Hashable, order-independent form of a shared-argument dict (lists become tuples)."""
+    return tuple(sorted((k, tuple(v) if isinstance(v, list) else v) for k, v in args.items()))
+
+
 class ModelBuilder:
     """Accumulates bodies, joints and shapes in Python lists, then :meth:`finalize` s to a Model."""
 
     ShapeConfig = ShapeConfig
     JointDofConfig = JointDofConfig
+    ActuatorEntry = ActuatorEntry
 
     def __init__(self, up_axis: str = "z", gravity: float = -9.81):
         self.up_axis = "xyz".index(up_axis.lower()) if isinstance(up_axis, str) else int(up_axis)
@@ -182,6 +214,9 @@ class ModelBuilder:
         self.shape_collision_filter_pairs: set[tuple[int, int]] = set()
         self.joint_dof_count = 0
         self.joint_coord_count = 0
+        self.actuator_entries: dict[tuple, ActuatorEntry] = {}
+        """Actuator groups accumulated by :meth:`add_actuator`, keyed by controller class, delay presence, clamping classes
+        with their shared arguments and the controller's shared arguments."""
 
     # ------------------------------------------------------------------ counts
     @property
@@ -292,6 +327,7 @@ class ModelBuilder:
         self.articulation_world.extend([w] * builder.articulation_count)
         self.articulation_label.extend(builder.articulation_label)
         self.shape_collision_filter_pairs.update((a + s0, b + s0) for a, b in builder.shape_collision_filter_pairs)
+        self._merge_builder_actuators(builder, d0, c0)
         if tf is not None:
             # Rigidly move root-attached entities: bodies, world-attached joint anchors and static shapes.
             for b in range(b0, self.body_count):
@@ -306,6 +342,103 @@ class ModelBuilder:
             for s in range(s0, self.shape_count):
                 if self.shape_body[s] == -1:
                     self.shape_transform[s] = X.transform_mul(tf, self.shape_transform[s])
+
+    def _merge_builder_actuators(self, builder: "ModelBuilder", joint_dof_offset: int, joint_coord_offset: int) -> None:
+        """Append ``builder``'s actuator groups, dof indices shifted by the dof offset and position indices by the coordinate
+        offset (reference ``ModelBuilder._merge_builder_actuators``)."""
+        for key, sub in builder.actuator_entries.items():
+            entry = self.actuator_entries.setdefault(key, ActuatorEntry(sub.controller_class, sub.clamping_classes,
+                                                                        sub.clamping_shared_kwargs, sub.controller_shared_kwargs))
+            entry.indices.extend(i + joint_dof_offset for i in sub.indices)
+            entry.pos_indices.extend(i + joint_coord_offset for i in sub.pos_indices)
+            entry.controller_args.extend(sub.controller_args)
+            entry.delay_args.extend(sub.delay_args)
+            entry.clamping_args.extend(sub.clamping_args)
+
+    # ------------------------------------------------------------------ actuators
+    def add_actuator(self, controller_class: type | None = None, index: int | None = None, clamping: list | None = None,
+                     delay_steps: int | None = None, pos_index: int | None = None, **kwargs: Any) -> None:
+        """Add an actuator for one dof (reference ``ModelBuilder.add_actuator``).
+
+        Calls with the same controller class, the same presence of a delay, the same clamping classes with equal shared
+        arguments and equal shared controller arguments accumulate into one :class:`~newton_b200.actuators.Actuator` at
+        :meth:`finalize`; different delays share a group, whose buffer is sized to the largest.
+
+        Args:
+            controller_class: e.g. :class:`~newton_b200.actuators.ControllerPD`.
+            index: dof index into ``joint_qd``-shaped arrays (velocities, velocity targets, feedforward, forces).
+            clamping: list of ``(ClampingClass, kwargs)`` applied after the controller, in order.
+            delay_steps: optional input delay [actuator steps].
+            pos_index: index into ``joint_q``-shaped arrays; defaults to ``index`` (differs from it behind a FREE or BALL joint).
+            **kwargs: per-dof controller parameters (e.g. ``kp``, ``kd``); unrecognised ones are ignored with a warning.
+        """
+        if controller_class is None:
+            raise TypeError("add_actuator() requires 'controller_class'")
+        if index is None:
+            raise TypeError("add_actuator() missing required argument: 'index'")
+        if delay_steps is not None:
+            from ..actuators import Delay
+
+            delay_steps = Delay.resolve_arguments({"delay_steps": delay_steps})["delay_steps"]
+        ctrl_args = controller_class.resolve_arguments(kwargs)
+        ignored = sorted(set(kwargs).difference(ctrl_args))
+        if ignored:
+            warnings.warn(f"add_actuator: {controller_class.__name__} ignoring unrecognized parameter(s): {', '.join(ignored)}",
+                          stacklevel=2)
+        ctrl_group, ctrl_own = _split_shared(controller_class, ctrl_args)
+        clamps = [(cls, *_split_shared(cls, cls.resolve_arguments(kw))) for cls, kw in clamping or ()]
+        # actuators share a group when everything but their per-dof values agrees
+        group = (controller_class, delay_steps is not None, tuple((cls, _frozen(shared)) for cls, shared, _ in clamps),
+                 _frozen(ctrl_group))
+        entry = self.actuator_entries.get(group)
+        if entry is None:
+            entry = self.actuator_entries[group] = ActuatorEntry(
+                controller_class, tuple(cls for cls, _, _ in clamps), tuple(shared for _, shared, _ in clamps), ctrl_group)
+        entry.indices.append(index)
+        entry.pos_indices.append(index if pos_index is None else pos_index)
+        entry.controller_args.append(ctrl_own)
+        entry.clamping_args.append([own for _, _, own in clamps])
+        if delay_steps is not None:
+            entry.delay_args.append({"delay_steps": delay_steps})
+
+    @staticmethod
+    def _stack_args(args_list: list[dict], device, integer: bool = False) -> dict:
+        """Per-actuator argument dicts -> one ``(N,)`` tensor per key: float32, or int32 for integer delay steps."""
+        out = {}
+        for key in args_list[0].keys() if args_list else ():
+            values = [a[key] for a in args_list]
+            for v in values:
+                if not isinstance(v, int | float):
+                    raise TypeError(f"add_actuator expects scalar per-DOF params, but parameter '{key}' got {type(v).__name__}; "
+                                    f"pass one scalar per add_actuator call")
+            if integer and all(isinstance(v, int) for v in values):
+                out[key] = torch.tensor(values, dtype=torch.int32, device=device)
+            else:
+                out[key] = torch.from_numpy(np.asarray(values, dtype=np.float32)).to(device)
+        return out
+
+    def _finalize_actuators(self, m: Model) -> None:
+        """``Model.actuators``, one :class:`~newton_b200.actuators.Actuator` per group (reference ``finalize``)."""
+        from ..actuators import Actuator, Delay
+
+        dev = m.device
+        m.actuators = []
+        for entry in self.actuator_entries.values():
+            indices = torch.tensor(entry.indices, dtype=torch.int32, device=dev)
+            pos_indices = None
+            if entry.pos_indices != entry.indices:
+                pos_indices = torch.tensor(entry.pos_indices, dtype=torch.int32, device=dev)
+            controller = entry.controller_class(**self._stack_args(entry.controller_args, dev), **entry.controller_shared_kwargs)
+            delay = None
+            if entry.delay_args:
+                delay = Delay(**self._stack_args(entry.delay_args, dev, integer=True),
+                              max_delay=max(a["delay_steps"] for a in entry.delay_args))
+            clamps = []
+            for k, (cc, shared) in enumerate(zip(entry.clamping_classes, entry.clamping_shared_kwargs, strict=True)):
+                clamps.append(cc(**self._stack_args([per[k] for per in entry.clamping_args], dev), **shared))
+            target_pos_indices = pos_indices if (pos_indices is not None and m.use_coord_layout_targets) else indices
+            m.actuators.append(Actuator(indices=indices, controller=controller, delay=delay, clamping=clamps or None,
+                                        pos_indices=pos_indices, target_pos_indices=target_pos_indices))
 
     # ------------------------------------------------------------------ bodies
     def add_link(self, *, xform=None, com=None, inertia=None, mass=0.0, label=None, lock_inertia=False,
@@ -965,4 +1098,5 @@ class ModelBuilder:
         gv = [*self.world_gravity, g] if (self.world_gravity and not implicit_world) else [g for _ in range(W)]
         m.gravity = arr(gv, (3,), F32)
         m.bvh_build_shapes(m)  # ray-casting shape tables for the initial state, as upstream's finalize does
+        self._finalize_actuators(m)
         return m

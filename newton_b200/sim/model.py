@@ -326,6 +326,7 @@ class Model:
         self.bvh_shape_group_start = None  # [W+2] int32: group g's entries of bvh_shape_enabled; group W = global world -1
         self.bvh_shape_world_transforms = None  # [S,7] world transform of every shape, as of the last refit
         self.bvh_shape_bounds = None  # [S,2,3] unscaled local bounds of mesh-backed shapes (MAXVAL / -MAXVAL for the others)
+        self.actuators: list = []  # newton_b200.actuators.Actuator groups built by ModelBuilder.finalize (reference Model.actuators)
         self._requested_contact_attributes: set[str] = set()
         self._requested_state_attributes: set[str] = set()
 
@@ -453,6 +454,8 @@ class Model:
                 setattr(out, k, moved.clone() if moved.data_ptr() == v.data_ptr() else moved)  # same device: still a copy
             elif k.startswith("_nb2_"):
                 continue  # per-model native caches (the nb2_model handle borrows THIS model's array addresses and device)
+            elif k == "actuators":
+                out.actuators = [a._rebuilt(out.device) for a in v]  # every parameter, index and table on the new device
             elif k != "device":
                 setattr(out, k, v.copy() if isinstance(v, (list, set, dict)) else v)
         # re-establish the aliasing of joint_target_q_start

@@ -130,6 +130,12 @@ def shard_model(model: Model, rank: int, world_size: int) -> Model:
     out.shape_contact_pairs = torch.from_numpy(remap.astype(np.int32)).to(model.device)
     out.shape_contact_pair_count = int(remap.shape[0])
     out.gravity = torch.cat([model.gravity[w0:w1], model.gravity[-1:]]).clone()
+    out.actuators = []
+    for act in getattr(model, "actuators", []):  # the actuators of this slice's dofs, rebased; groups left empty are dropped
+        dof = act.indices.cpu().numpy()
+        keep = (dof >= d0) & (dof < d1)
+        if keep.any():
+            out.actuators.append(act._rebuilt(model.device, keep, d0, c0))
     if getattr(model, "bvh_shape_enabled", None) is not None:  # ray-casting tables for this slice, with the model's mask
         out.bvh_build_shapes(out, shape_flags=model._bvh_build_flags)
     return out
