@@ -483,6 +483,11 @@ static nb2_status upload_tables(nb2_model* m) {
     NB2_CUDA_CHECK(cudaMemset(p, 0, (size_t(dv.env_count) + 1) * sizeof(int)));
     m->allocations.push_back(p);
     dv.env_contact_offset = static_cast<int*>(p);
+    NB2_CUDA_CHECK(cudaMalloc(&p, 2 * (size_t(dv.env_count) + 1) * sizeof(int)));
+    NB2_CUDA_CHECK(cudaMemset(p, 0, 2 * (size_t(dv.env_count) + 1) * sizeof(int)));
+    m->allocations.push_back(p);
+    dv.collide_tile_count = static_cast<int*>(p);
+    dv.collide_tile_offset = dv.collide_tile_count + dv.env_count + 1;
     // tile chain of the fused contact export: ticket = done = 0, epoch = 1 (zeroed status words belong to epoch 0: invalid)
     NB2_CUDA_CHECK(cudaMalloc(&p, 4 * sizeof(int)));
     const int sync_init[4] = {0, 0, 1, 0};

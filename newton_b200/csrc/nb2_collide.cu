@@ -356,12 +356,22 @@ struct PairGeom {
     Xf X;
 };
 
-// Shared-memory record of one shape slot: world transform + expanded AABB.
+// Shared-memory record of one shape slot: world transform + expanded AABB, and the shape constants that the pair phase and the
+// write-out read, loaded once per slot in phase 1 instead of once per pair or contact behind a pair -> shape id chain of global
+// loads.  29 words: an odd stride, so lanes reading one field of different slots hit different banks.
 struct __align__(4) SlotRec {
     float x[7];
     float lo[3];
     float hi[3];
+    float scale[3];
+    float margin, gap;
+    float mu, mu_torsional, mu_rolling, ke, kd, kf, ka;  // contact material
+    int type;
+    int shape;      // model shape id
+    int body;       // model body id, -1 for static shapes
+    int immovable;  // static or kinematic body (read by the explicit list's immovable-pair filter only)
 };
+static_assert(sizeof(SlotRec) == 29 * 4, "SlotRec: keep the stride odd");
 
 // Write-out staging (DevModel::lane_per_contact): the narrow phase leaves a pair's candidates in the registers of ONE lane - the 4
 // contacts of a foot would be converted and stored by that lane one after the other while the group's other lanes idle.  Instead
@@ -372,7 +382,7 @@ struct __align__(4) StageContact {
     int pair_lane;
 };
 struct __align__(4) StagePair {
-    int sa, sb;
+    int ia, ib;  // slots
     float reff_a, reff_b, marg_a, marg_b;
 };
 __host__ __device__ inline size_t stage_bytes_per_group(int L) { return size_t(L) * 5 * sizeof(StageContact) + size_t(L) * sizeof(StagePair); }
@@ -394,7 +404,8 @@ NB2_DEV ShapeMotion ld_motion(const SlotMotionRec& r) {
 // nb2_model_create): the analytic-only kernel carries neither the MPR / GJK / manifold code nor its registers and stack.
 // WARPS warps per CTA (each warp = 32/L environments): the kernel is a straight line every warp walks once, so one-warp CTAs each
 // fetch the whole instruction stream cold (`stall_no_inst`); warps of one CTA
-// start together and share the fetches.
+// start together and share the fetches.  The generic 8-warp instantiation is held to two CTAs per SM (at most 128 registers; left
+// to itself ptxas takes 166 and one CTA fits): 4096 environments of 16 lanes are 256 CTAs, one wave on 132 SMs.
 // EXPORT = true also writes the reference-layout `Contacts` arrays in the same launch (the separate contact_export_kernel is gone from
 // the default path): a CTA ("tile") knows its environments' contact counts after the pair loop; the offset of its first contact in the
 // global arrays is the sum over all earlier tiles, obtained by a decoupled look-back over one status word per tile (epoch | flag |
@@ -402,7 +413,7 @@ NB2_DEV ShapeMotion ld_motion(const SlotMotionRec& r) {
 // waits on tiles that started before it; the last CTA to finish re-arms ticket / done and bumps the epoch, which makes the words of
 // the previous launch (or graph replay) invalid without a memset.  Integer sums: the offsets equal a serial scan's.
 template <int L, bool CONVEX, int WARPS, bool EXPORT>
-__global__ void __launch_bounds__(32 * WARPS) collide_kernel(DevModel M, const float* __restrict__ body_q, nb2_contacts_view out) {
+__global__ void __launch_bounds__(32 * WARPS, (CONVEX && WARPS > 1) ? 2 : 0) collide_kernel(DevModel M, const float* __restrict__ body_q, nb2_contacts_view out) {
     constexpr int G = 32 / L;  // environments per warp
     extern __shared__ unsigned char smem_raw[];
     __shared__ int s_tile[2];              // tile index, epoch
@@ -454,13 +465,16 @@ __global__ void __launch_bounds__(32 * WARPS) collide_kernel(DevModel M, const f
         }
         slot0 = M.env_slot_start[env];
     }
-    // ---- phase 1: transforms + AABBs -----------------------------------------------------------
+    // ---- phase 1: transforms + AABBs + shape constants -------------------------------------------
+    const bool immovable_filter = !M.include_static_kinematic_pairs && !M.dyn_pairs;
     for (int s = l; s < nslots; s += L) {
         int sid = s < nloc ? ss + s : M.global_shapes[s - nloc];
         int body = d.shape_body[sid];
         Xf X = ldx(d.shape_transform + 7 * sid);
         if (body != -1) X = xmul(ldx(body_q + 7 * body), X);
         float margin = d.shape_margin[sid];
+        const float gap = d.shape_gap[sid];
+        const V3 scale = ld3(d.shape_scale + 3 * sid);
         V3 lo, hi;
         const int stype = d.shape_type[sid];
         V3 llo, lhi;
@@ -468,10 +482,25 @@ __global__ void __launch_bounds__(32 * WARPS) collide_kernel(DevModel M, const f
             llo = ld3(d.shape_collision_aabb_lower + 3 * sid);
             lhi = ld3(d.shape_collision_aabb_upper + 3 * sid);
         }
-        shape_aabb(stype, ld3(d.shape_scale + 3 * sid), X, margin + d.shape_gap[sid], d.shape_collision_radius[sid], llo, lhi, lo, hi);
+        shape_aabb(stype, scale, X, margin + gap, d.shape_collision_radius[sid], llo, lhi, lo, hi);
+        SlotRec& r = slots[s];
+        st3(r.scale, scale);
+        r.margin = margin;
+        r.gap = gap;
+        r.mu = d.shape_material_mu[sid];
+        r.mu_torsional = d.shape_material_mu_torsional[sid];
+        r.mu_rolling = d.shape_material_mu_rolling[sid];
+        r.ke = d.shape_material_ke[sid];
+        r.kd = d.shape_material_kd[sid];
+        r.kf = d.shape_material_kf[sid];
+        r.ka = d.shape_material_ka[sid];
+        r.type = stype;
+        r.shape = sid;
+        r.body = body;
+        if (immovable_filter) r.immovable = body < 0 || (d.body_flags[body] & 2) != 0;
         if (CONVEX && motion) {
             ShapeMotion mo;
-            mo.search_gap = d.shape_gap[sid];
+            mo.search_gap = gap;
             if (spec_mode == 2) mo = shape_motion(M, body_q, sid, body, X, lo, hi);
             st3(motion[s].lin, mo.lin);
             st3(motion[s].ang, mo.ang);
@@ -495,7 +524,7 @@ __global__ void __launch_bounds__(32 * WARPS) collide_kernel(DevModel M, const f
         unsigned vmask = 0;  // bit i set -> contact candidate i of this pair is emitted
         float cdist[5];
         V3 cpos[5], cnorm[5];
-        int sa = 0, sb = 0;
+        int ia = 0, ib = 0;  // slots of the pair
         float reff_a = 0.f, reff_b = 0.f, marg_a = 0.f, marg_b = 0.f;
         int mesh_a = -1, mesh_b = -1;  // slots of an overlapping (mesh, infinite plane) pair: handled by the whole group below
         if (live && p < np) {
@@ -506,28 +535,25 @@ __global__ void __launch_bounds__(32 * WARPS) collide_kernel(DevModel M, const f
             bool overlap = alo.x <= bhi.x && ahi.x >= blo.x && alo.y <= bhi.y && ahi.y >= blo.y && alo.z <= bhi.z && ahi.z >= blo.z;
             if (CONVEX && spec_mode == 2)  // swept test over the relative displacement (the explicit sweep passes (s1, s2) = the stored pair)
                 overlap = aabb_overlap_moving(alo, ahi, blo, bhi, ld3(motion[pr.x].disp) - ld3(motion[pr.y].disp));
-            if (overlap && !M.include_static_kinematic_pairs && !M.dyn_pairs) {
-                // is_shape_pair_immovable_filtered (broad_phase_common.py:166-201) in the explicit sweep (broad_phase_nxn.py:29-69)
-                const int s1 = pr.x < nloc ? ss + pr.x : M.global_shapes[pr.x - nloc], s2 = pr.y < nloc ? ss + pr.y : M.global_shapes[pr.y - nloc];
-                const int b1 = d.shape_body[s1], b2 = d.shape_body[s2];
-                const bool im1 = b1 < 0 || (d.body_flags[b1] & 2) != 0, im2 = b2 < 0 || (d.body_flags[b2] & 2) != 0;
-                if (im1 && im2) overlap = false;
-            }
+            // is_shape_pair_immovable_filtered (broad_phase_common.py:166-201) in the explicit sweep (broad_phase_nxn.py:29-69)
+            if (overlap && immovable_filter && slots[pr.x].immovable && slots[pr.y].immovable) overlap = false;
             if (CONVEX && overlap && mesh_pair) {
                 mesh_a = pr.x;
                 mesh_b = pr.y;
                 overlap = false;
             }
             if (overlap) {
-                sa = pr.x < nloc ? ss + pr.x : M.global_shapes[pr.x - nloc];
-                sb = pr.y < nloc ? ss + pr.y : M.global_shapes[pr.y - nloc];
-                const int ta = d.shape_type[sa], tb = d.shape_type[sb];
-                V3 sca = ld3(d.shape_scale + 3 * sa), scb = ld3(d.shape_scale + 3 * sb);
-                Xf Xa = ldx(slots[pr.x].x), Xb = ldx(slots[pr.y].x);
-                marg_a = d.shape_margin[sa];
-                marg_b = d.shape_margin[sb];
+                const SlotRec &ra = slots[pr.x], &rb = slots[pr.y];
+                ia = pr.x;
+                ib = pr.y;
+                const int sa = ra.shape, sb = rb.shape;
+                const int ta = ra.type, tb = rb.type;
+                V3 sca = ld3(ra.scale), scb = ld3(rb.scale);
+                Xf Xa = ldx(ra.x), Xb = ldx(rb.x);
+                marg_a = ra.margin;
+                marg_b = rb.margin;
                 // speculative: the colliders see the velocity-extended search gaps, the admission test the authored ones
-                const float base_gap_sum = d.shape_gap[sa] + d.shape_gap[sb];
+                const float base_gap_sum = ra.gap + rb.gap;
                 const float gap_sum = (CONVEX && spec_mode == 2) ? motion[pr.x].search_gap + motion[pr.y].search_gap : base_gap_sum;
                 const bool early_gjk = ta >= GEO_ELLIPSOID || tb == GEO_CONE || (ta == GEO_CAPSULE && tb > GEO_CAPSULE);
                 bool analytic = false;
@@ -604,8 +630,8 @@ __global__ void __launch_bounds__(32 * WARPS) collide_kernel(DevModel M, const f
                         }
                     }
                 } else if (CONVEX) {
-                    ConvexShape A{ta, sca, Xa, marg_a, d.shape_gap[sa], alo, ahi};
-                    ConvexShape Bc{tb, scb, Xb, marg_b, d.shape_gap[sb], blo, bhi};
+                    ConvexShape A{ta, sca, Xa, marg_a, ra.gap, alo, ahi};
+                    ConvexShape Bc{tb, scb, Xb, marg_b, rb.gap, blo, bhi};
                     ConvexSpec cs;
                     if (spec_mode != 0) {
                         const ShapeMotion ma = ld_motion(motion[pr.x]), mb = ld_motion(motion[pr.y]);
@@ -662,7 +688,7 @@ __global__ void __launch_bounds__(32 * WARPS) collide_kernel(DevModel M, const f
             if (stage_c) {
                 if (cnt > 0) {
                     StagePair& sp = stage_p[l];
-                    sp.sa = sa; sp.sb = sb;
+                    sp.ia = ia; sp.ib = ib;
                     sp.reff_a = reff_a; sp.reff_b = reff_b; sp.marg_a = marg_a; sp.marg_b = marg_b;
                     int k = incl - cnt;
     #pragma unroll
@@ -681,9 +707,9 @@ __global__ void __launch_bounds__(32 * WARPS) collide_kernel(DevModel M, const f
                 for (int c = l; c < total; c += L) {
                     const StageContact& sc = stage_c[c];
                     const StagePair& sp = stage_p[sc.pair_lane];
-                    const int psa = sp.sa, psb = sp.sb;
+                    const SlotRec &sla = slots[sp.ia], &slb = slots[sp.ib];
                     const float ra = sp.reff_a, rb = sp.reff_b;
-                    const int body0 = d.shape_body[psa], body1 = d.shape_body[psb];
+                    const int body0 = sla.body, body1 = slb.body;
                     const Xf Xbw_a = body0 == -1 ? Xf() : xinv(ldx(body_q + 7 * body0));
                     const Xf Xbw_b = body1 == -1 ? Xf() : xinv(ldx(body_q + 7 * body1));
                     const int o = slot0 + n_total + c;
@@ -696,8 +722,8 @@ __global__ void __launch_bounds__(32 * WARPS) collide_kernel(DevModel M, const f
                     const V3 o0 = xvec(Xbw_a, om_a * n), o1 = xvec(Xbw_b, -om_b * n);
                     cb[CF_BODY_A * T + o] = __int_as_float(body0 >= 0 ? body0 - bs : -1);
                     cb[CF_BODY_B * T + o] = __int_as_float(body1 >= 0 ? body1 - bs : -1);
-                    cb[CF_SHAPE0 * T + o] = __int_as_float(psa);
-                    cb[CF_SHAPE1 * T + o] = __int_as_float(psb);
+                    cb[CF_SHAPE0 * T + o] = __int_as_float(sla.shape);
+                    cb[CF_SHAPE1 * T + o] = __int_as_float(slb.shape);
                     cb[CF_P0X * T + o] = p0.x; cb[CF_P0Y * T + o] = p0.y; cb[CF_P0Z * T + o] = p0.z;
                     cb[CF_P1X * T + o] = p1.x; cb[CF_P1Y * T + o] = p1.y; cb[CF_P1Z * T + o] = p1.z;
                     cb[CF_O0X * T + o] = o0.x; cb[CF_O0Y * T + o] = o0.y; cb[CF_O0Z * T + o] = o0.z;
@@ -705,26 +731,28 @@ __global__ void __launch_bounds__(32 * WARPS) collide_kernel(DevModel M, const f
                     cb[CF_NX * T + o] = n.x; cb[CF_NY * T + o] = n.y; cb[CF_NZ * T + o] = n.z;
                     cb[CF_MARGIN0 * T + o] = om_a;
                     cb[CF_MARGIN1 * T + o] = om_b;
-                    cb[CF_MU * T + o] = (d.shape_material_mu[psa] + d.shape_material_mu[psb]) / 2.0f;
-                    cb[CF_MU_TORSIONAL * T + o] = (d.shape_material_mu_torsional[psa] + d.shape_material_mu_torsional[psb]) / 2.0f;
-                    cb[CF_MU_ROLLING * T + o] = (d.shape_material_mu_rolling[psa] + d.shape_material_mu_rolling[psb]) / 2.0f;
-                    cb[CF_KE * T + o] = 0.5f * (d.shape_material_ke[psa] + d.shape_material_ke[psb]);
-                    cb[CF_KD * T + o] = 0.5f * (d.shape_material_kd[psa] + d.shape_material_kd[psb]);
-                    cb[CF_KF * T + o] = 0.5f * (d.shape_material_kf[psa] + d.shape_material_kf[psb]);
-                    cb[CF_KA * T + o] = 0.5f * (d.shape_material_ka[psa] + d.shape_material_ka[psb]);
+                    cb[CF_MU * T + o] = (sla.mu + slb.mu) / 2.0f;
+                    cb[CF_MU_TORSIONAL * T + o] = (sla.mu_torsional + slb.mu_torsional) / 2.0f;
+                    cb[CF_MU_ROLLING * T + o] = (sla.mu_rolling + slb.mu_rolling) / 2.0f;
+                    cb[CF_KE * T + o] = 0.5f * (sla.ke + slb.ke);
+                    cb[CF_KD * T + o] = 0.5f * (sla.kd + slb.kd);
+                    cb[CF_KF * T + o] = 0.5f * (sla.kf + slb.kf);
+                    cb[CF_KA * T + o] = 0.5f * (sla.ka + slb.ka);
                 }
                 __syncwarp();  // the staging area is rewritten in the next round
             } else if (cnt > 0) {
-                const int body0 = d.shape_body[sa], body1 = d.shape_body[sb];
+                const SlotRec &sla = slots[ia], &slb = slots[ib];
+                const int sa = sla.shape, sb = slb.shape;
+                const int body0 = sla.body, body1 = slb.body;
                 const Xf Xbw_a = body0 == -1 ? Xf() : xinv(ldx(body_q + 7 * body0));
                 const Xf Xbw_b = body1 == -1 ? Xf() : xinv(ldx(body_q + 7 * body1));
-                const float mu = (d.shape_material_mu[sa] + d.shape_material_mu[sb]) / 2.0f;
-                const float mut = (d.shape_material_mu_torsional[sa] + d.shape_material_mu_torsional[sb]) / 2.0f;
-                const float mur = (d.shape_material_mu_rolling[sa] + d.shape_material_mu_rolling[sb]) / 2.0f;
-                const float ke = 0.5f * (d.shape_material_ke[sa] + d.shape_material_ke[sb]);
-                const float kd = 0.5f * (d.shape_material_kd[sa] + d.shape_material_kd[sb]);
-                const float kf = 0.5f * (d.shape_material_kf[sa] + d.shape_material_kf[sb]);
-                const float ka = 0.5f * (d.shape_material_ka[sa] + d.shape_material_ka[sb]);
+                const float mu = (sla.mu + slb.mu) / 2.0f;
+                const float mut = (sla.mu_torsional + slb.mu_torsional) / 2.0f;
+                const float mur = (sla.mu_rolling + slb.mu_rolling) / 2.0f;
+                const float ke = 0.5f * (sla.ke + slb.ke);
+                const float kd = 0.5f * (sla.kd + slb.kd);
+                const float kf = 0.5f * (sla.kf + slb.kf);
+                const float ka = 0.5f * (sla.ka + slb.ka);
                 float* cb = M.cb;
                 const size_t T = size_t(M.slot_total);
     #pragma unroll
@@ -763,16 +791,17 @@ __global__ void __launch_bounds__(32 * WARPS) collide_kernel(DevModel M, const f
                 // ---- mesh vs infinite plane (narrow_phase.py:1761-1861, reduce_contacts=False): the group walks the vertices L at a
                 // time; a vertex within gap + margin of the plane is a contact (shape_a = mesh, normal mesh -> plane), kept in vertex order
                 const int ma = __shfl_sync(gmask, mesh_a, seg_hi, L), mb = __shfl_sync(gmask, mesh_b, seg_hi, L);
-                const int msa = ma < nloc ? ss + ma : M.global_shapes[ma - nloc], psb = mb < nloc ? ss + mb : M.global_shapes[mb - nloc];
-                const Xf Xm = ldx(slots[ma].x), Xp = ldx(slots[mb].x);
+                const SlotRec &slm = slots[ma], &slp = slots[mb];
+                const int msa = slm.shape, psb = slp.shape;
+                const Xf Xm = ldx(slm.x), Xp = ldx(slp.x);
                 const Xf Xp_inv = xinv(Xp);
                 const V3 pn = xvec(Xp, V3(0.f, 0.f, 1.f));
-                const V3 mscale = ld3(d.shape_scale + 3 * msa);
-                const float marg_m = d.shape_margin[msa], marg_p = d.shape_margin[psb];
-                const float gap_sum = d.shape_gap[msa] + d.shape_gap[psb];
+                const V3 mscale = ld3(slm.scale);
+                const float marg_m = slm.margin, marg_p = slp.margin;
+                const float gap_sum = slm.gap + slp.gap;
                 const float* verts = d.hull_points + 3 * size_t(d.shape_hull_start[msa]);
                 const int nv = d.shape_hull_count[msa];
-                const int body0 = d.shape_body[msa], body1 = d.shape_body[psb];
+                const int body0 = slm.body, body1 = slp.body;
                 const Xf Xbw_a = body0 == -1 ? Xf() : xinv(ldx(body_q + 7 * body0));
                 const Xf Xbw_b = body1 == -1 ? Xf() : xinv(ldx(body_q + 7 * body1));
                 float* cb = M.cb;
@@ -814,13 +843,13 @@ __global__ void __launch_bounds__(32 * WARPS) collide_kernel(DevModel M, const f
                         cb[CF_NX * T + o] = n.x; cb[CF_NY * T + o] = n.y; cb[CF_NZ * T + o] = n.z;
                         cb[CF_MARGIN0 * T + o] = om_a;
                         cb[CF_MARGIN1 * T + o] = om_b;
-                        cb[CF_MU * T + o] = (d.shape_material_mu[msa] + d.shape_material_mu[psb]) / 2.0f;
-                        cb[CF_MU_TORSIONAL * T + o] = (d.shape_material_mu_torsional[msa] + d.shape_material_mu_torsional[psb]) / 2.0f;
-                        cb[CF_MU_ROLLING * T + o] = (d.shape_material_mu_rolling[msa] + d.shape_material_mu_rolling[psb]) / 2.0f;
-                        cb[CF_KE * T + o] = 0.5f * (d.shape_material_ke[msa] + d.shape_material_ke[psb]);
-                        cb[CF_KD * T + o] = 0.5f * (d.shape_material_kd[msa] + d.shape_material_kd[psb]);
-                        cb[CF_KF * T + o] = 0.5f * (d.shape_material_kf[msa] + d.shape_material_kf[psb]);
-                        cb[CF_KA * T + o] = 0.5f * (d.shape_material_ka[msa] + d.shape_material_ka[psb]);
+                        cb[CF_MU * T + o] = (slm.mu + slp.mu) / 2.0f;
+                        cb[CF_MU_TORSIONAL * T + o] = (slm.mu_torsional + slp.mu_torsional) / 2.0f;
+                        cb[CF_MU_ROLLING * T + o] = (slm.mu_rolling + slp.mu_rolling) / 2.0f;
+                        cb[CF_KE * T + o] = 0.5f * (slm.ke + slp.ke);
+                        cb[CF_KD * T + o] = 0.5f * (slm.kd + slp.kd);
+                        cb[CF_KF * T + o] = 0.5f * (slm.kf + slp.kf);
+                        cb[CF_KA * T + o] = 0.5f * (slm.ka + slp.ka);
                     }
                     written += __popc(hits);
                 }
@@ -831,14 +860,23 @@ __global__ void __launch_bounds__(32 * WARPS) collide_kernel(DevModel M, const f
         }
     }
     if (live && l == 0) M.env_contact_count[env] = n_total;
-    if constexpr (!EXPORT) return;
+    constexpr int NE = WARPS * G;  // environments per tile (<= 32)
+    if (l == 0) s_off[warp * G + grp] = live ? n_total : 0;
+    __syncthreads();  // also makes this CTA's contact-block stores visible to the lanes that copy them out below (EXPORT)
+    if constexpr (!EXPORT) {
+        // the tile's total: contact_export_kernel takes its offsets from these and the per-environment counts
+        if (warp == 0) {
+            int total = lane < NE ? s_off[lane] : 0;
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) total += __shfl_xor_sync(0xffffffffu, total, o);
+            if (lane == 0) M.collide_tile_count[blockIdx.x] = total;
+        }
+        return;
+    }
 
     // ---- fused export: tile-local offsets, look-back for the tile base, scatter -----------------------------------------------
     typedef unsigned long long u64;
-    constexpr int NE = WARPS * G;  // environments per tile (<= 32)
     const unsigned epoch = unsigned(s_tile[1]) & 0x3FFFFFFFu;
-    if (l == 0) s_off[warp * G + grp] = live ? n_total : 0;
-    __syncthreads();  // also makes this CTA's contact-block stores visible to the lanes that copy them out below
     if (warp == 0) {
         const int mine = lane < NE ? s_off[lane] : 0;
         int incl = mine;
@@ -1090,7 +1128,7 @@ __global__ void __launch_bounds__(32) broadphase_kernel(DevModel M, const float*
 }
 
 // ---- export to the reference `Contacts` arrays ---------------------------------------------------
-// Single-CTA exclusive scan of the per-env counts (E <= a few 10^5), then one group per env scatters its block.
+// Single-CTA exclusive scan of the per-tile contact counts collide_kernel leaves (large batches; see contact_export_kernel).
 __global__ void __launch_bounds__(1024) contact_scan_kernel(const int* __restrict__ counts, int E, int* __restrict__ offsets,
                                                             int* __restrict__ rigid_contact_count) {
     __shared__ int warp_sums[32];
@@ -1131,58 +1169,100 @@ __global__ void __launch_bounds__(1024) contact_scan_kernel(const int* __restric
     }
 }
 
-// SELF_SCAN (batches up to 8192 environments): one pass - every CTA (4 environments, one warp each) first sums the contact
-// counts of all environments before its own (E/128 coalesced int loads per thread out of L2; exact integer arithmetic, so
-// the offsets equal the scan's) and then scatters its environments' contact blocks; this saves the single-CTA scan
-// launch.  The sum is O(E^2 / 128) over the grid, so larger batches keep the
-// separate contact_scan_kernel and read its offsets.
+// One CTA per EXPORT_ENVS consecutive environments: their contacts are one contiguous range of the output arrays.  The range
+// starts at (contacts of the collide CTAs before the one holding the first environment) + (contacts of that collide CTA's
+// environments before it); collide_kernel leaves both the per-environment and the per-CTA counts.  Integer sums: the offsets
+// equal a serial scan's.  SELF_SCAN (batches up to 8192 environments) sums the earlier collide CTAs' totals itself; larger
+// batches read contact_scan_kernel's scan of them.  The range is copied in chunks of EXPORT_CHUNK contacts: one thread per
+// contact gathers its slot from the contact blocks into shared memory, laid out like the output arrays, then every array is
+// written as consecutive words across the threads.
+constexpr int EXPORT_ENVS = 16, EXPORT_THREADS = 256, EXPORT_CHUNK = 256;
 template <bool SELF_SCAN>
-__global__ void __launch_bounds__(128) contact_export_kernel(DevModel M, nb2_contacts_view out) {
-    __shared__ int warp_part[4];
-    const int env0 = blockIdx.x * 4;
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    const int env = env0 + wid;
-    int dst0;
-    if (SELF_SCAN) {
-        int part = 0;
-        for (int i = threadIdx.x; i < env0; i += 128) part += M.env_contact_count[i];
+__global__ void __launch_bounds__(EXPORT_THREADS) contact_export_kernel(DevModel M, nb2_contacts_view out) {
+    __shared__ int s_part[EXPORT_THREADS / 32];
+    __shared__ int s_off[EXPORT_ENVS + 1];  // offsets of the CTA's environments inside its range; [EXPORT_ENVS] = range size
+    __shared__ int s_slot[EXPORT_ENVS];     // first contact-block slot of each environment
+    __shared__ int s_shape[2][EXPORT_CHUNK];
+    __shared__ float s_vec[5][3 * EXPORT_CHUNK];  // point0, point1, offset0, offset1, normal
+    __shared__ float s_margin[2][EXPORT_CHUNK];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int e0 = blockIdx.x * EXPORT_ENVS;
+    const int ne = min(EXPORT_ENVS, M.env_count - e0);
+    const int TE = M.collide_tile_envs, tile0 = e0 / TE;
+    int part = 0;
+    if (SELF_SCAN)
+        for (int i = tid; i < tile0; i += EXPORT_THREADS) part += M.collide_tile_count[i];
+    for (int e = tile0 * TE + tid; e < e0; e += EXPORT_THREADS) part += M.env_contact_count[e];
 #pragma unroll
-        for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
-        if (lane == 0) warp_part[wid] = part;
-        __syncthreads();
-        dst0 = warp_part[0] + warp_part[1] + warp_part[2] + warp_part[3];
-        for (int e = env0; e < env && e < M.env_count; ++e) dst0 += M.env_contact_count[e];
-    } else {
-        dst0 = env < M.env_count ? M.env_contact_offset[env] : 0;
-    }
-    if (env >= M.env_count) return;
-    const int n = M.env_contact_count[env];
-    if (SELF_SCAN && lane == 0) {
-        M.env_contact_offset[env] = dst0;
-        if (env == M.env_count - 1) {
-            M.env_contact_offset[M.env_count] = dst0 + n;
-            out.rigid_contact_count[0] = dst0 + n;
+    for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+    if (lane == 0) s_part[warp] = part;
+    __syncthreads();
+    int base = SELF_SCAN ? 0 : M.collide_tile_offset[tile0];
+#pragma unroll
+    for (int w = 0; w < EXPORT_THREADS / 32; ++w) base += s_part[w];
+    if (warp == 0) {
+        const int cnt = lane < ne ? M.env_contact_count[e0 + lane] : 0;
+        int incl = cnt;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int v = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += v;
+        }
+        if (lane < EXPORT_ENVS) s_off[lane] = incl - cnt;
+        if (lane == 31) s_off[EXPORT_ENVS] = incl;
+        if (lane < ne) {
+            s_slot[lane] = M.env_slot_start[e0 + lane];
+            M.env_contact_offset[e0 + lane] = base + incl - cnt;
+            if (e0 + lane == M.env_count - 1) {
+                M.env_contact_offset[M.env_count] = base + incl;
+                out.rigid_contact_count[0] = base + incl;
+            }
         }
     }
-    const int src0 = M.env_slot_start[env];
+    __syncthreads();
+    const int n = s_off[EXPORT_ENVS];
+    // overflow: the count keeps growing, the writes past rigid_contact_max are dropped (collide.py:176-177)
+    const int n_fit = max(0, min(n, out.rigid_contact_max - base));
     const size_t T = size_t(M.slot_total);
     const float* cb = M.cb;
-    for (int c = lane; c < n; c += 32) {
-        const int s = src0 + c, o = dst0 + c;
-        if (o >= out.rigid_contact_max) break;  // overflow: count keeps growing, writes dropped (collide.py:176-177)
-        out.shape0[o] = __float_as_int(cb[CF_SHAPE0 * T + s]);
-        out.shape1[o] = __float_as_int(cb[CF_SHAPE1 * T + s]);
+    for (int c0 = 0; c0 < n_fit; c0 += EXPORT_CHUNK) {
+        const int m = min(EXPORT_CHUNK, n_fit - c0);
+        if (tid < m) {
+            const int c = c0 + tid;
+            int j = 0;  // the environment holding contact c: the last one whose range starts at or before c
 #pragma unroll
-        for (int k = 0; k < 3; ++k) {
-            out.point0[3 * o + k] = cb[(CF_P0X + k) * T + s];
-            out.point1[3 * o + k] = cb[(CF_P1X + k) * T + s];
-            out.offset0[3 * o + k] = cb[(CF_O0X + k) * T + s];
-            out.offset1[3 * o + k] = cb[(CF_O1X + k) * T + s];
-            out.normal[3 * o + k] = cb[(CF_NX + k) * T + s];
+            for (int k = 1; k < EXPORT_ENVS; ++k) j += s_off[k] <= c ? 1 : 0;
+            const size_t s = size_t(s_slot[j]) + (c - s_off[j]);
+            s_shape[0][tid] = __float_as_int(cb[CF_SHAPE0 * T + s]);
+            s_shape[1][tid] = __float_as_int(cb[CF_SHAPE1 * T + s]);
+#pragma unroll
+            for (int k = 0; k < 3; ++k) {
+                s_vec[0][3 * tid + k] = cb[(CF_P0X + k) * T + s];
+                s_vec[1][3 * tid + k] = cb[(CF_P1X + k) * T + s];
+                s_vec[2][3 * tid + k] = cb[(CF_O0X + k) * T + s];
+                s_vec[3][3 * tid + k] = cb[(CF_O1X + k) * T + s];
+                s_vec[4][3 * tid + k] = cb[(CF_NX + k) * T + s];
+            }
+            s_margin[0][tid] = cb[CF_MARGIN0 * T + s];
+            s_margin[1][tid] = cb[CF_MARGIN1 * T + s];
         }
-        out.margin0[o] = cb[CF_MARGIN0 * T + s];
-        out.margin1[o] = cb[CF_MARGIN1 * T + s];
-        if (out.tids) out.tids[o] = 0;
+        __syncthreads();
+        const size_t o0 = size_t(base) + c0;
+        for (int k = tid; k < m; k += EXPORT_THREADS) {
+            out.shape0[o0 + k] = s_shape[0][k];
+            out.shape1[o0 + k] = s_shape[1][k];
+            out.margin0[o0 + k] = s_margin[0][k];
+            out.margin1[o0 + k] = s_margin[1][k];
+            if (out.tids) out.tids[o0 + k] = 0;
+        }
+        for (int k = tid; k < 3 * m; k += EXPORT_THREADS) {
+            out.point0[3 * o0 + k] = s_vec[0][k];
+            out.point1[3 * o0 + k] = s_vec[1][k];
+            out.offset0[3 * o0 + k] = s_vec[2][k];
+            out.offset1[3 * o0 + k] = s_vec[3][k];
+            out.normal[3 * o0 + k] = s_vec[4][k];
+        }
+        __syncthreads();  // the staging area is refilled by the next chunk
     }
 }
 
@@ -1393,8 +1473,9 @@ nb2_status launch_contacts_import(nb2_model* m, const nb2_contacts_view& in, cud
 
 template <int L, bool CONVEX, int WARPS>
 static nb2_status launch_collide_W(nb2_model* m, const float* body_q, const nb2_contacts_view* fused_out, cudaStream_t s) {
-    const DevModel& M = m->dev;
     const int NE = (32 / L) * WARPS;
+    m->dev.collide_tile_envs = NE;
+    const DevModel& M = m->dev;
     const int blocks = (M.env_count + NE - 1) / NE;
     const size_t smem = size_t(NE) * M.max_env_slots_shapes * (sizeof(SlotRec) + (CONVEX && M.spec_mode != 0 ? sizeof(SlotMotionRec) : 0)) +
                         (M.lane_per_contact ? size_t(NE) * stage_bytes_per_group(L) : 0);
@@ -1494,12 +1575,14 @@ nb2_status launch_collide(nb2_model* m, const float* body_q, const nb2_contacts_
 #undef NB2_COLLIDE_DISPATCH
     if (st != NB2_OK) return st;
     if (contacts && !fused_out) {
+        const int blocks = (M.env_count + EXPORT_ENVS - 1) / EXPORT_ENVS;
         if (M.env_count <= 8192) {
-            contact_export_kernel<true><<<(M.env_count + 3) / 4, 128, 0, s>>>(M, *contacts);
+            contact_export_kernel<true><<<blocks, EXPORT_THREADS, 0, s>>>(M, *contacts);
             count_launch();
         } else {
-            contact_scan_kernel<<<1, 1024, 0, s>>>(M.env_contact_count, M.env_count, M.env_contact_offset, contacts->rigid_contact_count);
-            contact_export_kernel<false><<<(M.env_count + 3) / 4, 128, 0, s>>>(M, *contacts);
+            const int tiles = (M.env_count + M.collide_tile_envs - 1) / M.collide_tile_envs;
+            contact_scan_kernel<<<1, 1024, 0, s>>>(M.collide_tile_count, tiles, M.collide_tile_offset, nullptr);
+            contact_export_kernel<false><<<blocks, EXPORT_THREADS, 0, s>>>(M, *contacts);
             count_launch(2);
         }
         NB2_CUDA_CHECK(cudaGetLastError());

@@ -47,6 +47,9 @@ struct DevModel {
     int slot_total;
     int* env_contact_count;        // [E]
     int* env_contact_offset;       // [E+1] exclusive scan, written by the export path
+    int* collide_tile_count;       // [E+1] contacts found by each collide_kernel CTA ("tile")
+    int* collide_tile_offset;      // [E+1] exclusive scan of collide_tile_count (large batches: contact_scan_kernel)
+    int collide_tile_envs;         // environments per collide_kernel CTA of the last launch
     int* collide_sync;             // [3] ticket / done / epoch of the fused export's tile chain (collide_kernel)
     unsigned long long* collide_tile_status;  // [E] (epoch | flag | count) per tile: decoupled look-back of the export offsets
     int max_env_bodies, max_env_joints, max_env_slots_shapes, max_env_pairs, max_env_contact_slots;
