@@ -567,6 +567,64 @@ nb2_status nb2_actuator_param_gather(const int32_t* map, int32_t entries, const 
 nb2_status nb2_actuator_param_scatter(const int32_t* map, int32_t entries, int32_t dofs_per_world, const uint8_t* world_mask,
                                       const void* values, void* param, int32_t is_int, void* cuda_stream);
 
+/* --- inverse kinematics (reference newton.ik, sim/ik/) ----------------------------------------------------------------------
+ * Batched Levenberg-Marquardt IK over one articulated model: `n_batch` independent rows (problems x seeds) share the model and
+ * the objective list.  nb2_ik_solve runs every LM iteration of every row in ONE launch (a sub-warp group of lanes per row, all
+ * intermediates in shared memory) and closes with the cost evaluation of IKSolver.step.  The descriptor borrows the model's
+ * joint / body arrays directly (no nb2_model handle); the objective tables are built on the host at IKSolver construction.
+ * Nothing is allocated and nothing synchronises the host, so the calls can be captured in a CUDA graph. */
+#define NB2_IK_MAX_OBJECTIVES 16
+enum { NB2_IK_POSITION = 1, NB2_IK_ROTATION = 2, NB2_IK_JOINT_LIMIT = 3 };
+enum { NB2_IK_ANALYTIC = 0, NB2_IK_MIXED = 1 };
+enum { NB2_IK_SAMPLE_NONE = 0, NB2_IK_SAMPLE_GAUSS = 1, NB2_IK_SAMPLE_ROBERTS = 2, NB2_IK_SAMPLE_UNIFORM = 3 };
+
+typedef struct nb2_ik_objective {
+    int32_t kind;               /* NB2_IK_* */
+    int32_t row;                /* first residual row of the objective */
+    int32_t link;               /* body index (position / rotation) */
+    int32_t canonicalize;       /* rotation: flip q_err onto the short arc */
+    float weight;
+    float offset[4];            /* position: link_offset (x, y, z); rotation: link_offset_rotation (x, y, z, w) */
+    const float* target;        /* position [n_problems, 3] / rotation [n_problems, 4] (x, y, z, w) */
+    const float* limit_lower;   /* joint limit [joint_dof_count] */
+    const float* limit_upper;
+    const uint8_t* affects_dof; /* position / rotation [joint_dof_count]: 1 where the dof's joint is an ancestor of `link` */
+} nb2_ik_objective;
+
+typedef struct nb2_ik_desc {
+    nb2_model_desc model;       /* the articulation: joint / body arrays and counts (shape arrays are not read) */
+    int32_t mode;               /* NB2_IK_ANALYTIC / NB2_IK_MIXED */
+    int32_t n_batch;            /* expanded rows = n_problems * n_seeds */
+    int32_t n_seeds;
+    int32_t n_residuals;
+    int32_t objective_count;
+    int32_t lanes;              /* lanes per row (8 / 16 / 32); 0 = chosen from the joint and dof counts */
+    const int32_t* dof_to_coord;/* [joint_dof_count] coordinate of dof k of joint j = joint_q_start[j] + k */
+    const int32_t* fk_level;    /* MIXED [joint_count]: schedule level of the joint's FK step, -1 = not evaluated */
+    int32_t fk_level_count;
+    const uint8_t* dof_mask;    /* [joint_dof_count] 0 = column fixed at zero; NULL = every dof optimised */
+    float lambda_initial, lambda_factor, lambda_min, lambda_max, rho_min;
+    nb2_ik_objective objectives[NB2_IK_MAX_OBJECTIVES];
+} nb2_ik_desc;
+
+/* The LM solve of IKSolver.step (ik_lm_optimizer.py:509-705 + the closing compute_costs, ik_solver.py:383).  `joint_q_in`
+ * [n_batch, coords] is read once, `joint_q` [n_batch, coords] receives the solution (may alias joint_q_in); `joint_q_out`
+ * (optional, may alias) receives a second copy.  residuals / costs are those of the final configuration, lambda_values and
+ * jacobian those of the last iteration (jacobian is left untouched when iterations == 0).  write_lambda = 0 leaves
+ * lambda_values alone (IKOptimizerLM.compute_costs is iterations = 0, write_lambda = 0).  `seed_state` (optional) is
+ * incremented once by the launch, the device-side counter advance of IKSolver._pull_seed. */
+nb2_status nb2_ik_solve(const nb2_ik_desc* desc, const float* joint_q_in, float* joint_q, float* joint_q_out, float* residuals,
+                        float* costs, float* lambda_values, float* jacobian, int32_t iterations, float step_size, int32_t write_lambda,
+                        uint32_t* seed_state, void* cuda_stream);
+/* IKSolver._sample (ik_solver.py:48-141): fills joint_q_expanded [n_problems * n_seeds, coords] from joint_q_in
+ * [n_problems, coords] with `sampler`; the bound tables are [coords] (bounded: 0/1).  Reads seed_state[0] (not advanced). */
+nb2_status nb2_ik_sample(int32_t sampler, int32_t n_problems, int32_t n_seeds, int32_t n_coords, const float* joint_q_in,
+                         const float* lower, const float* upper, const int32_t* bounded, const float* roberts_basis, float noise_std,
+                         const uint32_t* seed_state, float* joint_q_expanded, void* cuda_stream);
+/* _select_best_seed_indices + _gather_best_seed (ik_solver.py:144-176): the lowest cost per problem, first seed on ties. */
+nb2_status nb2_ik_select(int32_t n_problems, int32_t n_seeds, int32_t n_coords, const float* costs, const float* joint_q_expanded,
+                         int32_t* best, float* joint_q_out, void* cuda_stream);
+
 /* --- multi-GPU end-of-frame state gather without compute kernels (SURVEY.md §8(e)) --------------------------------------
  * Replaces the `ncclAllGather(body_q, body_qd)` of the reference design (there is no reference code for it: upstream is
  * single-GPU; the sharding follows sim/model.py:1081-1097 world ranges).  Every rank owns a receive buffer of

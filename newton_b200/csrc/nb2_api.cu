@@ -1014,6 +1014,85 @@ nb2_status nb2_intersect_ray(const nb2_raycast_view* view, int32_t ray_count, co
                                 out_normal, static_cast<cudaStream_t>(cuda_stream));
 }
 
+nb2_status nb2_ik_solve(const nb2_ik_desc* desc, const float* joint_q_in, float* joint_q, float* joint_q_out, float* residuals,
+                        float* costs, float* lambda_values, float* jacobian, int32_t iterations, float step_size, int32_t write_lambda,
+                        uint32_t* seed_state, void* cuda_stream) {
+    if (!desc) {
+        set_error("nb2_ik_solve: NULL descriptor");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    const nb2_ik_desc& d = *desc;
+    const nb2_model_desc& m = d.model;
+    if (d.n_batch < 0 || d.n_seeds < 1 || iterations < 0 || d.objective_count < 0 || d.objective_count > NB2_IK_MAX_OBJECTIVES ||
+        d.n_residuals < 0 || (d.mode != NB2_IK_ANALYTIC && d.mode != NB2_IK_MIXED) ||
+        (d.lanes != 0 && d.lanes != 8 && d.lanes != 16 && d.lanes != 32)) {
+        set_error("nb2_ik_solve: invalid n_batch, n_seeds, iterations, objective_count, n_residuals, mode or lanes");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    if (d.n_batch == 0) return NB2_OK;
+    if (!joint_q_in || !joint_q || !residuals || !costs || !lambda_values || (iterations > 0 && d.n_residuals > 0 && !jacobian) ||
+        !d.dof_to_coord || !m.joint_type || !m.joint_parent || !m.joint_child || !m.joint_q_start || !m.joint_qd_start || !m.joint_dof_dim ||
+        !m.joint_X_p || !m.joint_X_c || !m.body_com || !m.body_flags || (m.joint_dof_count > 0 && !m.joint_axis) ||
+        (d.mode == NB2_IK_MIXED && !d.fk_level)) {
+        set_error("nb2_ik_solve: NULL state, output or model array");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    int rows = 0;
+    for (int i = 0; i < d.objective_count; ++i) {
+        const nb2_ik_objective& o = d.objectives[i];
+        const int dim = o.kind == NB2_IK_JOINT_LIMIT ? m.joint_dof_count : 3;
+        const bool ok = (o.kind == NB2_IK_POSITION || o.kind == NB2_IK_ROTATION)
+                            ? (o.target && o.affects_dof && o.link >= 0 && o.link < m.body_count)
+                            : (o.kind == NB2_IK_JOINT_LIMIT && (m.joint_dof_count == 0 || (o.limit_lower && o.limit_upper)));
+        if (!ok || o.row != rows) {
+            set_error("nb2_ik_solve: objective " + std::to_string(i) + " has an unknown kind, NULL tables, a link out of range or a row " +
+                      "that does not follow the previous objective's");
+            return NB2_ERR_INVALID_ARGUMENT;
+        }
+        rows += dim;
+    }
+    if (rows != d.n_residuals) {
+        set_error("nb2_ik_solve: the objectives hold " + std::to_string(rows) + " residual rows, n_residuals is " + std::to_string(d.n_residuals));
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    return launch_ik_solve(d, joint_q_in, joint_q, joint_q_out, residuals, costs, lambda_values, jacobian, iterations, step_size, write_lambda,
+                           seed_state, static_cast<cudaStream_t>(cuda_stream));
+}
+
+nb2_status nb2_ik_sample(int32_t sampler, int32_t n_problems, int32_t n_seeds, int32_t n_coords, const float* joint_q_in, const float* lower,
+                         const float* upper, const int32_t* bounded, const float* roberts_basis, float noise_std, const uint32_t* seed_state,
+                         float* joint_q_expanded, void* cuda_stream) {
+    if (sampler < NB2_IK_SAMPLE_NONE || sampler > NB2_IK_SAMPLE_UNIFORM || n_problems < 0 || n_seeds < 1 || n_coords < 0) {
+        set_error("nb2_ik_sample: invalid sampler, n_problems, n_seeds or n_coords");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    if (n_problems == 0 || n_coords == 0) return NB2_OK;
+    const bool need_in = sampler == NB2_IK_SAMPLE_NONE || sampler == NB2_IK_SAMPLE_GAUSS;
+    const bool need_bounds = sampler != NB2_IK_SAMPLE_NONE;
+    if (!joint_q_expanded || (need_in && !joint_q_in) || (need_bounds && (!lower || !upper || !bounded)) ||
+        (sampler == NB2_IK_SAMPLE_ROBERTS && !roberts_basis) ||
+        ((sampler == NB2_IK_SAMPLE_GAUSS || sampler == NB2_IK_SAMPLE_UNIFORM) && !seed_state)) {
+        set_error("nb2_ik_sample: NULL array for the requested sampler");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    return launch_ik_sample(sampler, n_problems, n_seeds, n_coords, joint_q_in, lower, upper, bounded, roberts_basis, noise_std, seed_state,
+                            joint_q_expanded, static_cast<cudaStream_t>(cuda_stream));
+}
+
+nb2_status nb2_ik_select(int32_t n_problems, int32_t n_seeds, int32_t n_coords, const float* costs, const float* joint_q_expanded,
+                         int32_t* best, float* joint_q_out, void* cuda_stream) {
+    if (n_problems < 0 || n_seeds < 1 || n_coords < 0) {
+        set_error("nb2_ik_select: invalid n_problems, n_seeds or n_coords");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    if (n_problems == 0) return NB2_OK;
+    if (!costs || !joint_q_expanded || !joint_q_out) {
+        set_error("nb2_ik_select: NULL costs, joint_q_expanded or joint_q_out");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    return launch_ik_select(n_problems, n_seeds, n_coords, costs, joint_q_expanded, best, joint_q_out, static_cast<cudaStream_t>(cuda_stream));
+}
+
 nb2_status nb2_actuator_step(const nb2_actuator_step_desc* desc, void* cuda_stream) {
     if (!desc) {
         set_error("nb2_actuator_step: NULL descriptor");

@@ -14,7 +14,7 @@
 // The public functions use the COM-referenced world-twist convention (J @ joint_qd == body_qd), not the solve-origin
 // convention of featherstone_step_kernel, so none of that kernel's scratch is reused here.
 #include "nb2_internal.cuh"
-#include "nb2_spatial.cuh"
+#include "nb2_joint.cuh"
 
 namespace nb2 {
 namespace {
@@ -102,50 +102,11 @@ __device__ Xf parent_anchor(const nb2_model_desc& d, const float* body_q, int j)
 // jcalc_motion_subspace / write_free_distance_motion_subspace (sim/articulation.py:934-1069) for local joint k, and the world
 // COM of its child (the x_com_world of eval_articulation_jacobian :1153).  ROD columns stay zero (:1011-1013).
 __device__ void jacobian_subspace(const nb2_model_desc& d, const float* body_q, const float* joint_q, const Art& t, int k, DynSmem& s) {
-    const int j = t.j0 + k, type = d.joint_type[j], child = d.joint_child[j];
-    const int qs = d.joint_q_start[j], qds = d.joint_qd_start[j], lin = d.joint_dof_dim[2 * j], ang = d.joint_dof_dim[2 * j + 1];
+    const int j = t.j0 + k, child = d.joint_child[j];
     const Xf X_wpj = parent_anchor(d, body_q, j);
     const V3 xc = xpoint(ldx(body_q + 7 * child), ld3(d.body_com + 3 * child));
     st3(s.xcom + 3 * k, xc);
-    float* S = s.S + 6 * (qds - t.d0);
-    for (int q = 0; q < 6 * (d.joint_qd_start[j + 1] - qds); ++q) S[q] = 0.0f;
-    auto axis = [&](int i) { return ld3(d.joint_axis + 3 * i); };
-    if (type == FJ_PRISMATIC) {
-        st6(S, twist_xf(X_wpj, S6(axis(qds), V3())));
-    } else if (type == FJ_REVOLUTE) {
-        st6(S, twist_xf(X_wpj, S6(V3(), axis(qds))));
-    } else if (type == FJ_D6) {
-        for (int i = 0; i < 3; ++i)
-            if (lin > i) st6(S + 6 * i, twist_xf(X_wpj, S6(axis(qds + i), V3())));
-        const int iqd = qds + lin, iq = qs + lin;
-        float* Sa = S + 6 * lin;
-        if (ang == 1) st6(Sa, twist_xf(X_wpj, S6(V3(), axis(iqd))));
-        if (ang == 2) {
-            V3 a0, a1;
-            axes2(axis(iqd), axis(iqd + 1), joint_q[iq], a0, a1);
-            st6(Sa, twist_xf(X_wpj, S6(V3(), a0)));
-            st6(Sa + 6, twist_xf(X_wpj, S6(V3(), a1)));
-        }
-        if (ang == 3) {
-            V3 a0, a1, a2;
-            axes3(axis(iqd), axis(iqd + 1), axis(iqd + 2), joint_q[iq], joint_q[iq + 1], a0, a1, a2);
-            st6(Sa, twist_xf(X_wpj, S6(V3(), a0)));
-            st6(Sa + 6, twist_xf(X_wpj, S6(V3(), a1)));
-            st6(Sa + 12, twist_xf(X_wpj, S6(V3(), a2)));
-        }
-    } else if (type == FJ_BALL) {
-        st6(S, twist_xf(X_wpj, S6(V3(), V3(1.f, 0.f, 0.f))));
-        st6(S + 6, twist_xf(X_wpj, S6(V3(), V3(0.f, 1.f, 0.f))));
-        st6(S + 12, twist_xf(X_wpj, S6(V3(), V3(0.f, 0.f, 1.f))));
-    } else if (type == FJ_FREE || type == FJ_DISTANCE) {
-        const V3 ax = xvec(X_wpj, V3(1.f, 0.f, 0.f)), ay = xvec(X_wpj, V3(0.f, 1.f, 0.f)), az = xvec(X_wpj, V3(0.f, 0.f, 1.f));
-        st6(S, S6(ax, V3()));
-        st6(S + 6, S6(ay, V3()));
-        st6(S + 12, S6(az, V3()));
-        st6(S + 18, S6(-cross(ax, xc), ax));
-        st6(S + 24, S6(-cross(ay, xc), ay));
-        st6(S + 30, S6(-cross(az, xc), az));
-    }
+    joint_subspace(d, X_wpj, xc, joint_q, j, s.S + 6 * (d.joint_qd_start[j] - t.d0));
 }
 
 // J[6i + k][col] of eval_articulation_jacobian (:1148-1168): S_com of column col when the joint owning it is link i's joint or one

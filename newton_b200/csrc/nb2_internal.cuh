@@ -192,6 +192,14 @@ nb2_status launch_actuator_reset(int count, int buf_depth, const uint8_t* mask, 
                                  int* num_pushes, int* write_idx, float* integral, cudaStream_t s);
 nb2_status launch_actuator_param(bool gather, const int* map, int entries, int dofs_per_world, const uint8_t* world_mask, const void* src,
                                  void* dst, bool is_int, cudaStream_t s);
+nb2_status launch_ik_solve(const nb2_ik_desc& desc, const float* joint_q_in, float* joint_q, float* joint_q_out, float* residuals, float* costs,
+                           float* lambda_values, float* jacobian, int iterations, float step_size, int write_lambda, unsigned* seed_state,
+                           cudaStream_t s);
+nb2_status launch_ik_sample(int sampler, int n_problems, int n_seeds, int n_coords, const float* joint_q_in, const float* lower,
+                            const float* upper, const int* bounded, const float* basis, float noise_std, const unsigned* seed_state,
+                            float* out, cudaStream_t s);
+nb2_status launch_ik_select(int n_problems, int n_seeds, int n_coords, const float* costs, const float* joint_q_expanded, int* best,
+                            float* out, cudaStream_t s);
 }  // namespace nb2
 
 #define NB2_CUDA_CHECK(expr)                                                                          \

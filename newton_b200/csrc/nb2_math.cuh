@@ -69,12 +69,14 @@ NB2_DEV float acos_w(float x) { return (float)acos((double)x); }
 NB2_DEV float sin_w(float x) { return (float)sin((double)x); }
 NB2_DEV float cos_w(float x) { return (float)cos((double)x); }
 NB2_DEV float atan2_w(float y, float x) { return (float)atan2((double)y, (double)x); }
+NB2_DEV float log_w(float x) { return (float)log((double)x); }
 #else
 NB2_DEV float asin_w(float x) { return asinf(x); }
 NB2_DEV float acos_w(float x) { return acosf(x); }
 NB2_DEV float sin_w(float x) { return sinf(x); }
 NB2_DEV float cos_w(float x) { return cosf(x); }
 NB2_DEV float atan2_w(float y, float x) { return atan2f(y, x); }
+NB2_DEV float log_w(float x) { return logf(x); }
 #endif
 
 struct Q4 {

@@ -508,3 +508,37 @@ def range_ring_rays(model, body_q):
     origins = p[:, None, :].expand(-1, RANGE_RING_RAYS, -1).reshape(-1, 3).contiguous()
     worlds = torch.arange(model.world_count, device=body_q.device, dtype=torch.int32).repeat_interleave(RANGE_RING_RAYS)
     return origins, directions, worlds
+
+
+# Franka Emika Panda, from its published modified Denavit-Hartenberg table and joint ranges (a, d, alpha of frame i-1 -> i, metres /
+# radians) - 7 revolute joints, a fixed hand 0.107 m past the flange turned by -pi/4, two prismatic fingers 0.0584 m ahead of it.
+PANDA_DH = ((0.0, 0.333, 0.0), (0.0, 0.0, -0.5 * math.pi), (0.0, 0.316, 0.5 * math.pi), (0.0825, 0.0, 0.5 * math.pi),
+            (-0.0825, 0.384, -0.5 * math.pi), (0.0, 0.0, 0.5 * math.pi), (0.088, 0.0, 0.5 * math.pi))
+PANDA_LIMITS = ((-2.8973, 2.8973), (-1.7628, 1.7628), (-2.8973, 2.8973), (-3.0718, -0.0698), (-2.8973, 2.8973), (-0.0175, 3.7525),
+                (-2.8973, 2.8973))
+PANDA_HOME = (0.0, -0.785, 0.0, -2.356, 0.0, 1.571, 0.785, 0.02, 0.02)
+
+
+def panda_arm_model(device="cpu"):
+    """One Panda-class arm for inverse kinematics: 10 bodies / 10 joints (7 revolute, 1 fixed hand, 2 prismatic fingers), 9 dofs,
+    joint j driving body j (the layout the analytic IK mode needs).  Body 7 is the hand; ``joint_q`` starts at ``PANDA_HOME``."""
+    b = ModelBuilder()
+    inertia = np.eye(3) * 0.01
+    parent = -1
+    for i, ((a, d, alpha), (lo, hi)) in enumerate(zip(PANDA_DH, PANDA_LIMITS)):
+        rot = X.quat_from_axis_angle((1.0, 0.0, 0.0), alpha)
+        pos = np.array([a, 0.0, 0.0]) + X.quat_rotate(rot, np.array([0.0, 0.0, d]))
+        link = b.add_link(mass=1.0, inertia=inertia, label=f"panda/link{i + 1}")
+        b.add_joint_revolute(parent, link, parent_xform=X.transform(pos, rot), axis=(0.0, 0.0, 1.0), limit_lower=lo, limit_upper=hi,
+                             label=f"panda/joint{i + 1}")
+        parent = link
+    hand = b.add_link(mass=0.7, inertia=inertia, label="panda/hand")
+    b.add_joint_fixed(parent, hand, parent_xform=X.transform((0.0, 0.0, 0.107), X.quat_from_axis_angle((0.0, 0.0, 1.0), -0.25 * math.pi)),
+                      label="panda/hand_joint")
+    for side in (1.0, -1.0):
+        f = b.add_link(mass=0.015, inertia=inertia * 0.01, label=f"panda/finger{'_left' if side > 0 else '_right'}")
+        b.add_joint_prismatic(hand, f, parent_xform=X.transform((0.0, 0.0, 0.0584)), axis=(0.0, side, 0.0), limit_lower=0.0,
+                              limit_upper=0.04, label=f"panda/finger_joint{1 if side > 0 else 2}")
+    b.add_articulation(list(range(b.joint_count)), label="panda")
+    b.joint_q = list(PANDA_HOME)
+    return _finish(b, device)
