@@ -9,6 +9,7 @@
 #include <atomic>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <mutex>
 
 #include <cmath>
@@ -35,14 +36,14 @@ static nb2_status fetch(const T* dptr, size_t n, std::vector<T>& out) {
     return NB2_OK;
 }
 
+// Copies a host table into a new device buffer of at least one element; `buf` and `*out` change only on success.
 template <typename T>
-static nb2_status upload(nb2_model* m, const std::vector<T>& v, const T** out) {
-    void* p = nullptr;
-    size_t bytes = std::max<size_t>(v.size(), 1) * sizeof(T);
-    NB2_CUDA_CHECK(cudaMalloc(&p, bytes));
-    m->allocations.push_back(p);
-    if (!v.empty()) NB2_CUDA_CHECK(cudaMemcpy(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
-    *out = static_cast<const T*>(p);
+static nb2_status upload(const std::vector<T>& v, DeviceBuffer& buf, const T** out) {
+    DeviceBuffer fresh;
+    if (nb2_status st = fresh.alloc(std::max<size_t>(v.size(), 1) * sizeof(T))) return st;
+    if (!v.empty()) NB2_CUDA_CHECK(cudaMemcpy(fresh.get(), v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
+    buf = std::move(fresh);
+    *out = buf.get<const T>();
     return NB2_OK;
 }
 
@@ -394,16 +395,14 @@ static nb2_status build_tables(nb2_model* m, const nb2_model_desc& d) {
     dv.d = d;
     dv.env_count = E;
     dv.global_shape_count = int(h.global_shapes.size());
-    dv.max_env_bodies = dv.max_env_joints = dv.max_env_slots_shapes = dv.max_env_pairs = dv.max_env_contact_slots = 0;
+    dv.max_env_bodies = dv.max_env_joints = dv.max_env_slots_shapes = dv.max_env_pairs = 0;
     for (int e = 0; e < E; ++e) {
         dv.max_env_bodies = std::max(dv.max_env_bodies, h.env_body_start[e + 1] - h.env_body_start[e]);
         dv.max_env_joints = std::max(dv.max_env_joints, h.env_joint_start[e + 1] - h.env_joint_start[e]);
         dv.max_env_slots_shapes =
             std::max(dv.max_env_slots_shapes, h.env_shape_start[e + 1] - h.env_shape_start[e] + dv.global_shape_count);
         dv.max_env_pairs = std::max(dv.max_env_pairs, h.env_pair_start[e + 1] - h.env_pair_start[e]);
-        dv.max_env_contact_slots = std::max(dv.max_env_contact_slots, h.env_slot_start[e + 1] - h.env_slot_start[e]);
     }
-    dv.slot_total = h.env_slot_start[E];
     dv.has_mesh_pairs = m->has_mesh_pairs ? 1 : 0;
     m->lanes_per_env =
         std::min(32, std::max(8, pow2_at_least(std::max({dv.max_env_bodies, dv.max_env_joints, std::min(dv.max_env_pairs, 32)}))));
@@ -420,148 +419,97 @@ static nb2_status build_tables(nb2_model* m, const nb2_model_desc& d) {
     return NB2_OK;
 }
 
-static void free_allocations(nb2_model* m) {
-    for (void* p : m->allocations) cudaFree(p);
-    m->allocations.clear();
+// Contact blocks for the slot ranges `slot_start`: 5 slots per explicit pair (one per vertex of a mesh-plane pair), or per
+// candidate-capacity pair of the run-time broad phases.  Every buffer is allocated before the model changes, so a failed call
+// leaves it as it was.
+static nb2_status allocate_contact_blocks(nb2_model* m, std::vector<int> slot_start) {
+    DevModel& dv = m->dev;
+    const int E = dv.env_count;
+    DeviceBuffer slot_buf, impulse, cb;
+    const int* slot_ptr = nullptr;
+    nb2_status st;
+    if ((st = upload(slot_start, slot_buf, &slot_ptr))) return st;
+    if ((st = impulse.alloc(std::max<size_t>(size_t(slot_start[E]) * 6, 1) * sizeof(float), true))) return st;
+    if ((st = cb.alloc(std::max<size_t>(size_t(slot_start[E]) * CF_COUNT, 1) * sizeof(float), true))) return st;
+    NB2_CUDA_CHECK(cudaMemset(dv.env_contact_count, 0, (size_t(E) + 1) * sizeof(int)));
+    dv.max_env_contact_slots = 0;
+    for (int e = 0; e < E; ++e) dv.max_env_contact_slots = std::max(dv.max_env_contact_slots, slot_start[e + 1] - slot_start[e]);
+    dv.slot_total = slot_start[E];
+    m->env_slot_start = std::move(slot_buf);
+    m->contact_impulse = std::move(impulse);
+    m->cb = std::move(cb);
+    dv.env_slot_start = slot_ptr;
+    dv.contact_impulse = m->contact_impulse.get<float>();
+    dv.cb = m->cb.get<float>();
+    m->host.env_slot_start = std::move(slot_start);
+    return NB2_OK;
 }
 
 static nb2_status upload_tables(nb2_model* m) {
     HostTables& h = m->host;
     DevModel& dv = m->dev;
+    const size_t E1 = size_t(dv.env_count) + 1;
     nb2_status st;
-    if ((st = upload(m, h.env_body_start, &dv.env_body_start))) return st;
-    if ((st = upload(m, h.env_joint_start, &dv.env_joint_start))) return st;
-    if ((st = upload(m, h.env_shape_start, &dv.env_shape_start))) return st;
-    if ((st = upload(m, h.env_pair_start, &dv.env_pair_start))) return st;
-    if ((st = upload(m, h.env_slot_start, &dv.env_slot_start))) return st;
-    if ((st = upload(m, h.env_art_start, &dv.env_art_start))) return st;
-    if ((st = upload(m, h.global_shapes, &dv.global_shapes))) return st;
-    if ((st = upload(m, h.pairs, &dv.pairs))) return st;
-    if ((st = upload(m, h.body_joint_start, &dv.body_joint_start))) return st;
-    if ((st = upload(m, h.body_joint_entry, &dv.body_joint_entry))) return st;
-    if ((st = upload(m, h.joint_depth, &dv.joint_depth))) return st;
-    if ((st = upload(m, h.joint_anc_mask, &dv.joint_anc_mask))) return st;
-    if ((st = upload(m, h.art_H_start, &dv.art_H_start))) return st;
-    if ((st = upload(m, h.env_H_start, &dv.env_H_start))) return st;
-    if ((st = upload(m, h.art_batch_count, &dv.art_batch_count))) return st;
-    if ((st = upload(m, h.art_hb_body_start, &dv.art_hb_body_start))) return st;
-    if ((st = upload(m, h.art_hb_row_start, &dv.art_hb_row_start))) return st;
-    if ((st = upload(m, h.hb_body_col, &dv.hb_body_col))) return st;
-    if ((st = upload(m, h.hb_row_col, &dv.hb_row_col))) return st;
-    if ((st = upload(m, h.joint_desc_mask, &dv.joint_desc_mask))) return st;
-    if ((st = upload(m, h.dof_joint, &dv.dof_joint))) return st;
-    void* p = nullptr;
-    {
-        size_t nL = std::max<size_t>(size_t(h.env_H_start.back()), 1);
-        NB2_CUDA_CHECK(cudaMalloc(&p, nL * sizeof(float)));
-        NB2_CUDA_CHECK(cudaMemset(p, 0, nL * sizeof(float)));
-        m->allocations.push_back(p);
-        dv.fs_L = static_cast<float*>(p);
-    }
-    {
-        size_t n = std::max<size_t>(size_t(dv.slot_total) * 6, 1) * sizeof(float);
-        NB2_CUDA_CHECK(cudaMalloc(&p, n));
-        NB2_CUDA_CHECK(cudaMemset(p, 0, n));
-        m->allocations.push_back(p);
-        dv.contact_impulse = static_cast<float*>(p);
-        n = std::max<size_t>(size_t(dv.d.joint_count) * 6, 1) * sizeof(float);
-        NB2_CUDA_CHECK(cudaMalloc(&p, n));
-        NB2_CUDA_CHECK(cudaMemset(p, 0, n));
-        m->allocations.push_back(p);
-        dv.joint_impulse = static_cast<float*>(p);
-    }
-    size_t cb_bytes = std::max<size_t>(size_t(dv.slot_total) * CF_COUNT, 1) * sizeof(float);
-    NB2_CUDA_CHECK(cudaMalloc(&p, cb_bytes));
-    NB2_CUDA_CHECK(cudaMemset(p, 0, cb_bytes));
-    m->allocations.push_back(p);
-    dv.cb = static_cast<float*>(p);
-    NB2_CUDA_CHECK(cudaMalloc(&p, (size_t(dv.env_count) + 1) * sizeof(int)));
-    NB2_CUDA_CHECK(cudaMemset(p, 0, (size_t(dv.env_count) + 1) * sizeof(int)));
-    m->allocations.push_back(p);
-    dv.env_contact_count = static_cast<int*>(p);
-    NB2_CUDA_CHECK(cudaMalloc(&p, (size_t(dv.env_count) + 1) * sizeof(int)));
-    NB2_CUDA_CHECK(cudaMemset(p, 0, (size_t(dv.env_count) + 1) * sizeof(int)));
-    m->allocations.push_back(p);
-    dv.env_contact_offset = static_cast<int*>(p);
-    NB2_CUDA_CHECK(cudaMalloc(&p, 2 * (size_t(dv.env_count) + 1) * sizeof(int)));
-    NB2_CUDA_CHECK(cudaMemset(p, 0, 2 * (size_t(dv.env_count) + 1) * sizeof(int)));
-    m->allocations.push_back(p);
-    dv.collide_tile_count = static_cast<int*>(p);
-    dv.collide_tile_offset = dv.collide_tile_count + dv.env_count + 1;
+    if ((st = upload(h.env_body_start, m->env_body_start, &dv.env_body_start))) return st;
+    if ((st = upload(h.env_joint_start, m->env_joint_start, &dv.env_joint_start))) return st;
+    if ((st = upload(h.env_shape_start, m->env_shape_start, &dv.env_shape_start))) return st;
+    if ((st = upload(h.env_pair_start, m->env_pair_start, &dv.env_pair_start))) return st;
+    if ((st = upload(h.env_art_start, m->env_art_start, &dv.env_art_start))) return st;
+    if ((st = upload(h.global_shapes, m->global_shapes, &dv.global_shapes))) return st;
+    if ((st = upload(h.pairs, m->pairs, &dv.pairs))) return st;
+    if ((st = upload(h.body_joint_start, m->body_joint_start, &dv.body_joint_start))) return st;
+    if ((st = upload(h.body_joint_entry, m->body_joint_entry, &dv.body_joint_entry))) return st;
+    if ((st = upload(h.joint_depth, m->joint_depth, &dv.joint_depth))) return st;
+    if ((st = upload(h.joint_anc_mask, m->joint_anc_mask, &dv.joint_anc_mask))) return st;
+    if ((st = upload(h.art_H_start, m->art_H_start, &dv.art_H_start))) return st;
+    if ((st = upload(h.env_H_start, m->env_H_start, &dv.env_H_start))) return st;
+    if ((st = upload(h.art_batch_count, m->art_batch_count, &dv.art_batch_count))) return st;
+    if ((st = upload(h.art_hb_body_start, m->art_hb_body_start, &dv.art_hb_body_start))) return st;
+    if ((st = upload(h.art_hb_row_start, m->art_hb_row_start, &dv.art_hb_row_start))) return st;
+    if ((st = upload(h.hb_body_col, m->hb_body_col, &dv.hb_body_col))) return st;
+    if ((st = upload(h.hb_row_col, m->hb_row_col, &dv.hb_row_col))) return st;
+    if ((st = upload(h.joint_desc_mask, m->joint_desc_mask, &dv.joint_desc_mask))) return st;
+    if ((st = upload(h.dof_joint, m->dof_joint, &dv.dof_joint))) return st;
+    if ((st = m->fs_L.alloc(std::max<size_t>(size_t(h.env_H_start.back()), 1) * sizeof(float), true))) return st;
+    dv.fs_L = m->fs_L.get<float>();
+    if ((st = m->joint_impulse.alloc(std::max<size_t>(size_t(dv.d.joint_count) * 6, 1) * sizeof(float), true))) return st;
+    dv.joint_impulse = m->joint_impulse.get<float>();
+    if ((st = m->env_contact_count.alloc(E1 * sizeof(int), true))) return st;
+    dv.env_contact_count = m->env_contact_count.get<int>();
+    if ((st = m->env_contact_offset.alloc(E1 * sizeof(int), true))) return st;
+    dv.env_contact_offset = m->env_contact_offset.get<int>();
+    if ((st = m->collide_tile_count.alloc(2 * E1 * sizeof(int), true))) return st;
+    dv.collide_tile_count = m->collide_tile_count.get<int>();
+    dv.collide_tile_offset = dv.collide_tile_count + E1;
     // tile chain of the fused contact export: ticket = done = 0, epoch = 1 (zeroed status words belong to epoch 0: invalid)
-    NB2_CUDA_CHECK(cudaMalloc(&p, 4 * sizeof(int)));
+    if ((st = m->collide_sync.alloc(4 * sizeof(int)))) return st;
     const int sync_init[4] = {0, 0, 1, 0};
-    NB2_CUDA_CHECK(cudaMemcpy(p, sync_init, sizeof(sync_init), cudaMemcpyHostToDevice));
-    m->allocations.push_back(p);
-    dv.collide_sync = static_cast<int*>(p);
-    NB2_CUDA_CHECK(cudaMalloc(&p, std::max<size_t>(size_t(dv.env_count), 1) * sizeof(unsigned long long)));
-    NB2_CUDA_CHECK(cudaMemset(p, 0, std::max<size_t>(size_t(dv.env_count), 1) * sizeof(unsigned long long)));
-    m->allocations.push_back(p);
-    dv.collide_tile_status = static_cast<unsigned long long*>(p);
-    return NB2_OK;
-}
-
-
-// Frees one tracked device allocation (the contact blocks are re-sized when the broad phase changes).
-static void release(nb2_model* m, const void* p) {
-    if (!p) return;
-    for (size_t i = 0; i < m->allocations.size(); ++i)
-        if (m->allocations[i] == p) {
-            cudaFree(m->allocations[i]);
-            m->allocations.erase(m->allocations.begin() + i);
-            return;
-        }
-}
-
-// Contact-block slot ranges + buffers for the current pair source: 5 slots per explicit pair, or per candidate-capacity pair of
-// the run-time broad phases.
-static nb2_status allocate_contact_blocks(nb2_model* m) {
-    DevModel& dv = m->dev;
-    HostTables& h = m->host;
-    const int E = dv.env_count;
-    release(m, dv.env_slot_start);
-    release(m, dv.cb);
-    release(m, dv.contact_impulse);
-    dv.max_env_contact_slots = 0;
-    for (int e = 0; e < E; ++e) dv.max_env_contact_slots = std::max(dv.max_env_contact_slots, h.env_slot_start[e + 1] - h.env_slot_start[e]);
-    dv.slot_total = h.env_slot_start[E];
-    nb2_status st;
-    if ((st = upload(m, h.env_slot_start, &dv.env_slot_start))) return st;
-    void* p = nullptr;
-    size_t n = std::max<size_t>(size_t(dv.slot_total) * 6, 1) * sizeof(float);
-    NB2_CUDA_CHECK(cudaMalloc(&p, n));
-    NB2_CUDA_CHECK(cudaMemset(p, 0, n));
-    m->allocations.push_back(p);
-    dv.contact_impulse = static_cast<float*>(p);
-    n = std::max<size_t>(size_t(dv.slot_total) * CF_COUNT, 1) * sizeof(float);
-    NB2_CUDA_CHECK(cudaMalloc(&p, n));
-    NB2_CUDA_CHECK(cudaMemset(p, 0, n));
-    m->allocations.push_back(p);
-    dv.cb = static_cast<float*>(p);
-    NB2_CUDA_CHECK(cudaMemset(dv.env_contact_count, 0, (size_t(E) + 1) * sizeof(int)));
-    return NB2_OK;
+    NB2_CUDA_CHECK(cudaMemcpy(m->collide_sync.get(), sync_init, sizeof(sync_init), cudaMemcpyHostToDevice));
+    dv.collide_sync = m->collide_sync.get<int>();
+    if ((st = m->collide_tile_status.alloc(std::max<size_t>(size_t(dv.env_count), 1) * sizeof(unsigned long long), true))) return st;
+    dv.collide_tile_status = m->collide_tile_status.get<unsigned long long>();
+    return allocate_contact_blocks(m, h.env_slot_start);
 }
 
 static nb2_status configure_broad_phase(nb2_model* m, int mode, int max_pairs, bool include_static_kinematic) {
     DevModel& dv = m->dev;
     HostTables& h = m->host;
     const int E = dv.env_count;
-    dv.include_static_kinematic_pairs = include_static_kinematic ? 1 : 0;
-    if (mode == dv.broad_phase && (mode == NB2_BROAD_PHASE_EXPLICIT || max_pairs == m->dyn_pairs_requested)) return NB2_OK;
-    release(m, dv.dyn_pairs);
-    release(m, dv.env_dyn_count);
-    dv.dyn_pairs = nullptr;
-    dv.env_dyn_count = nullptr;
-    dv.dyn_pair_cap = 0;
+    if (mode == dv.broad_phase && (mode == NB2_BROAD_PHASE_EXPLICIT || max_pairs == m->dyn_pairs_requested)) {
+        dv.include_static_kinematic_pairs = include_static_kinematic ? 1 : 0;
+        return NB2_OK;
+    }
     if (mode != NB2_BROAD_PHASE_EXPLICIT && m->has_mesh_pairs) {
         set_error("nb2_collide_configure: MESH shapes are supported with the explicit broad phase only");
         return NB2_ERR_UNSUPPORTED;
     }
-    if (mode == NB2_BROAD_PHASE_EXPLICIT) {
-        h.env_slot_start = h.explicit_env_slot_start;  // 5 per pair, one per vertex for mesh-plane pairs
-        m->max_env_contacts = m->explicit_max_env_contacts;
-        m->has_convex_pairs = m->explicit_has_convex_pairs;
-    } else {
+    // the new configuration is built in locals and committed once every buffer exists
+    std::vector<int> slot_start = h.explicit_env_slot_start;  // 5 per pair, one per vertex for mesh-plane pairs
+    int cap = 0, max_env_contacts = m->explicit_max_env_contacts, filter_count = 0;
+    bool has_convex_pairs = m->explicit_has_convex_pairs;
+    DeviceBuffer dyn_pairs, env_dyn_count, filter_keys;
+    const long long* filter_ptr = nullptr;
+    if (mode != NB2_BROAD_PHASE_EXPLICIT) {
         if (dv.max_env_slots_shapes > 65535) {
             set_error("nb2_collide_configure: more than 65535 shapes in one world");
             return NB2_ERR_CAPACITY;
@@ -570,7 +518,6 @@ static nb2_status configure_broad_phase(nb2_model* m, int mode, int max_pairs, b
             set_error("nb2_collide_configure: broad_phase nxn / sap needs model.shape_collision_group");
             return NB2_ERR_INVALID_ARGUMENT;
         }
-        int cap = 0;
         std::vector<int> caps(size_t(E), 0);
         for (int e = 0; e < E; ++e) {
             const long long ns = h.env_shape_start[e + 1] - h.env_shape_start[e] + dv.global_shape_count;
@@ -579,30 +526,20 @@ static nb2_status configure_broad_phase(nb2_model* m, int mode, int max_pairs, b
             caps[e] = int(std::min<long long>(c, 1 << 20));
             cap = std::max(cap, caps[e]);
         }
-        for (int e = 0; e < E; ++e) h.env_slot_start[e + 1] = h.env_slot_start[e] + 5 * caps[e];
-        if (h.env_slot_start[E] < 0 || (long long)E * cap > (1ll << 30)) {
+        for (int e = 0; e < E; ++e) slot_start[e + 1] = slot_start[e] + 5 * caps[e];
+        if (slot_start[E] < 0 || (long long)E * cap > (1ll << 30)) {
             set_error("nb2_collide_configure: candidate capacity too large; pass max_pairs_per_world (CollisionPipeline(shape_pairs_max=...))");
             return NB2_ERR_CAPACITY;
         }
-        dv.dyn_pair_cap = cap;
-        void* p = nullptr;
-        NB2_CUDA_CHECK(cudaMalloc(&p, std::max<size_t>(size_t(E) * cap, 1) * sizeof(int2)));
-        m->allocations.push_back(p);
-        dv.dyn_pairs = static_cast<int2*>(p);
-        NB2_CUDA_CHECK(cudaMalloc(&p, (size_t(E) + 1) * sizeof(int)));
-        NB2_CUDA_CHECK(cudaMemset(p, 0, (size_t(E) + 1) * sizeof(int)));
-        m->allocations.push_back(p);
-        dv.env_dyn_count = static_cast<int*>(p);
-        m->max_env_contacts = 5 * cap;
-        m->has_convex_pairs = true;  // any type pair may show up at run time
+        nb2_status st;
+        if ((st = dyn_pairs.alloc(std::max<size_t>(size_t(E) * cap, 1) * sizeof(int2)))) return st;
+        if ((st = env_dyn_count.alloc((size_t(E) + 1) * sizeof(int), true))) return st;
+        max_env_contacts = 5 * cap;
+        has_convex_pairs = true;  // any type pair may show up at run time
         // excluded pairs -> sorted 64-bit keys
-        release(m, dv.filter_keys);
-        dv.filter_keys = nullptr;
-        dv.filter_count = 0;
         if (dv.d.shape_collision_filter_pair_count > 0 && dv.d.shape_collision_filter_pairs) {
             std::vector<int> fp;
-            nb2_status st = fetch(dv.d.shape_collision_filter_pairs, size_t(dv.d.shape_collision_filter_pair_count) * 2, fp);
-            if (st != NB2_OK) return st;
+            if ((st = fetch(dv.d.shape_collision_filter_pairs, size_t(dv.d.shape_collision_filter_pair_count) * 2, fp))) return st;
             std::vector<long long> keys;
             keys.reserve(fp.size() / 2);
             for (size_t i = 0; i + 1 < fp.size(); i += 2) {
@@ -611,29 +548,26 @@ static nb2_status configure_broad_phase(nb2_model* m, int mode, int max_pairs, b
             }
             std::sort(keys.begin(), keys.end());
             keys.erase(std::unique(keys.begin(), keys.end()), keys.end());
-            const long long* dk = nullptr;
-            if ((st = upload(m, keys, &dk))) return st;
-            dv.filter_keys = dk;
-            dv.filter_count = int(keys.size());
+            if ((st = upload(keys, filter_keys, &filter_ptr))) return st;
+            filter_count = int(keys.size());
         }
     }
+    if (nb2_status st = allocate_contact_blocks(m, std::move(slot_start))) return st;
+    m->dyn_pairs = std::move(dyn_pairs);
+    m->env_dyn_count = std::move(env_dyn_count);
+    m->filter_keys = std::move(filter_keys);
+    dv.dyn_pairs = m->dyn_pairs.get<int2>();
+    dv.env_dyn_count = m->env_dyn_count.get<int>();
+    dv.dyn_pair_cap = cap;
+    dv.filter_keys = filter_ptr;  // read by the run-time broad phases only
+    dv.filter_count = filter_count;
+    dv.include_static_kinematic_pairs = include_static_kinematic ? 1 : 0;
     dv.broad_phase = mode;
+    m->max_env_contacts = max_env_contacts;
+    m->has_convex_pairs = has_convex_pairs;
     m->dyn_pairs_requested = max_pairs;
-    return allocate_contact_blocks(m);
+    return NB2_OK;
 }
-
-// Every entry point runs on the model's device and leaves the caller's current device as it found it (a process may drive
-// several GPUs; nb2_model_destroy is called from a garbage collector at arbitrary points).
-struct DeviceGuard {
-    int prev = -1, dev = -1;
-    explicit DeviceGuard(int device) : dev(device) {
-        if (cudaGetDevice(&prev) != cudaSuccess) prev = -1;
-        if (prev != dev) cudaSetDevice(dev);
-    }
-    ~DeviceGuard() {
-        if (prev >= 0 && prev != dev) cudaSetDevice(prev);
-    }
-};
 
 }  // namespace nb2
 
@@ -648,30 +582,21 @@ nb2_status nb2_model_create(const nb2_model_desc* desc, int32_t device, nb2_mode
     }
     *out = nullptr;
     DeviceGuard guard(device);
-    nb2_model* m = new nb2_model();
+    std::unique_ptr<nb2_model> m(new nb2_model());
     m->device = device;
-    nb2_status st = build_tables(m, *desc);
-    if (st == NB2_OK) st = upload_tables(m);
-    if (st != NB2_OK) {
-        free_allocations(m);
-        delete m;
-        return st;
-    }
+    nb2_status st = build_tables(m.get(), *desc);
+    if (st == NB2_OK) st = upload_tables(m.get());
+    if (st != NB2_OK) return st;
     m->explicit_max_env_contacts = m->max_env_contacts;
     m->explicit_has_convex_pairs = m->has_convex_pairs;
     m->dev.include_static_kinematic_pairs = 1;
-    *out = m;
+    *out = m.release();
     return NB2_OK;
 }
 
 void nb2_model_destroy(nb2_model* model) {
     if (!model) return;
     DeviceGuard guard(model->device);
-    for (void* p : {(void*)model->match_new_keys, (void*)model->match_prev_keys, (void*)model->match_prev_claim, (void*)model->match_prev_pos,
-                    (void*)model->match_prev_normal, (void*)model->match_prev_count, (void*)model->match_prev_record,
-                    (void*)model->match_prev_was_matched})
-        if (p) cudaFree(p);
-    free_allocations(model);
     delete model;
 }
 

@@ -1326,33 +1326,31 @@ nb2_status launch_contacts_sort(nb2_model* m, const nb2_contacts_view& c, cudaSt
     while ((1ull << bits) <= (unsigned long long)m->dev.d.shape_count) ++bits;  // shape ids are 0 .. shape_count - 1
     const unsigned long long radix = 1ull << bits;
     const int end_bit = 2 * bits < 64 ? 2 * bits : 64;
-    if (C > m->sort_capacity) {
+    if (C > m->sort_capacity) {  // first use or a larger rigid_contact_max: new scratch (not capturable, see the header)
         size_t temp = 0;
         NB2_CUDA_CHECK(cub::DeviceRadixSort::SortPairs(nullptr, temp, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
                                                        (const int*)nullptr, (int*)nullptr, C, 0, end_bit, s));
-        void *k = nullptr, *ix = nullptr, *st = nullptr, *tmp = nullptr, *rk = nullptr;
-        NB2_CUDA_CHECK(cudaMalloc(&k, size_t(C) * 2 * sizeof(unsigned long long)));
-        NB2_CUDA_CHECK(cudaMalloc(&ix, size_t(C) * 2 * sizeof(int)));
-        NB2_CUDA_CHECK(cudaMalloc(&st, size_t(C) * 20 * sizeof(float)));
-        NB2_CUDA_CHECK(cudaMalloc(&rk, size_t(C) * sizeof(int)));
-        NB2_CUDA_CHECK(cudaMalloc(&tmp, std::max<size_t>(temp, 16)));
-        for (void* p : {k, ix, st, rk, tmp}) m->allocations.push_back(p);
-        m->sort_keys = static_cast<unsigned long long*>(k);
-        m->sort_keys_sorted = m->sort_keys + C;
-        m->sort_idx = static_cast<int*>(ix);
-        m->sort_idx_sorted = m->sort_idx + C;
-        m->sort_stage = static_cast<float*>(st);
-        m->sort_rank = static_cast<int*>(rk);
-        m->sort_temp = tmp;
-        m->sort_temp_bytes = temp;
+        DeviceBuffer k, ix, st, rk, tmp;
+        nb2_status e;
+        if ((e = k.alloc(size_t(C) * 2 * sizeof(unsigned long long))) || (e = ix.alloc(size_t(C) * 2 * sizeof(int))) ||
+            (e = st.alloc(size_t(C) * 20 * sizeof(float))) || (e = rk.alloc(size_t(C) * sizeof(int))) ||
+            (e = tmp.alloc(std::max<size_t>(temp, 16))))
+            return e;
+        m->replace_scratch(m->sort_keys, std::move(k));
+        m->replace_scratch(m->sort_idx, std::move(ix));
+        m->replace_scratch(m->sort_stage, std::move(st));
+        m->replace_scratch(m->sort_rank, std::move(rk));
+        m->replace_scratch(m->sort_temp, std::move(tmp));
         m->sort_capacity = C;
     }
-    sort_keys_kernel<<<(C + 255) / 256, 256, 0, s>>>(c, radix, m->sort_keys, m->sort_idx, m->sort_stage);
-    size_t temp = m->sort_temp_bytes;
-    NB2_CUDA_CHECK(cub::DeviceRadixSort::SortPairs(m->sort_temp, temp, m->sort_keys, m->sort_keys_sorted, m->sort_idx, m->sort_idx_sorted, C, 0,
-                                                   end_bit, s));  // stable
-    sort_gather_kernel<<<(C + 255) / 256, 256, 0, s>>>(c, m->sort_idx_sorted, m->sort_stage, m->sort_rank);
-    m->dev.export_rank = m->sort_rank;
+    unsigned long long* keys = m->sort_keys.get<unsigned long long>();
+    int* idx = m->sort_idx.get<int>();
+    sort_keys_kernel<<<(C + 255) / 256, 256, 0, s>>>(c, radix, keys, idx, m->sort_stage.get<float>());
+    size_t temp = m->sort_temp.bytes();
+    NB2_CUDA_CHECK(cub::DeviceRadixSort::SortPairs(m->sort_temp.get(), temp, keys, keys + m->sort_capacity, idx, idx + m->sort_capacity, C,
+                                                   0, end_bit, s));  // stable
+    sort_gather_kernel<<<(C + 255) / 256, 256, 0, s>>>(c, idx + m->sort_capacity, m->sort_stage.get<float>(), m->sort_rank.get<int>());
+    m->dev.export_rank = m->sort_rank.get<int>();
     count_launch(2);
     NB2_CUDA_CHECK(cudaGetLastError());
     return NB2_OK;
@@ -1441,31 +1439,26 @@ nb2_status launch_contacts_import(nb2_model* m, const nb2_contacts_view& in, cud
     const int C = in.rigid_contact_max;
     int end_bit = 1;
     while ((1 << end_bit) <= M.env_count) ++end_bit;  // keys are 0..env_count
-    if (C > m->import_capacity) {  // (re)allocate scratch: not capturable, see the header
+    if (C > m->import_capacity) {  // first use or a larger rigid_contact_max: new scratch (not capturable, see the header)
         size_t temp = 0;
         NB2_CUDA_CHECK(cub::DeviceRadixSort::SortPairs(nullptr, temp, (const int*)nullptr, (int*)nullptr, (const int*)nullptr, (int*)nullptr, C, 0,
                                                        end_bit, s));
-        int* buf = nullptr;
-        NB2_CUDA_CHECK(cudaMalloc(&buf, size_t(C) * 4 * sizeof(int)));
-        m->allocations.push_back(buf);
-        void* tmp = nullptr;
-        NB2_CUDA_CHECK(cudaMalloc(&tmp, std::max<size_t>(temp, 16)));
-        m->allocations.push_back(tmp);
-        m->import_keys = buf;
-        m->import_keys_sorted = buf + C;
-        m->import_idx = buf + 2 * size_t(C);
-        m->import_idx_sorted = buf + 3 * size_t(C);
-        m->import_temp = tmp;
-        m->import_temp_bytes = temp;
+        DeviceBuffer buf, tmp;
+        nb2_status e;
+        if ((e = buf.alloc(size_t(C) * 4 * sizeof(int))) || (e = tmp.alloc(std::max<size_t>(temp, 16)))) return e;
+        m->replace_scratch(m->import_buf, std::move(buf));
+        m->replace_scratch(m->import_temp, std::move(tmp));
         m->import_capacity = C;
     }
+    int* keys = m->import_buf.get<int>();  // [4][capacity]: keys, sorted keys, indices, sorted indices
+    const size_t cap = size_t(m->import_capacity);
     if (C > 0) {
-        import_keys_kernel<<<(C + 255) / 256, 256, 0, s>>>(M, in, m->implicit_single ? 1 : 0, m->import_keys, m->import_idx);
-        size_t temp = m->import_temp_bytes;
-        NB2_CUDA_CHECK(cub::DeviceRadixSort::SortPairs(m->import_temp, temp, m->import_keys, m->import_keys_sorted, m->import_idx,
-                                                       m->import_idx_sorted, C, 0, end_bit, s));  // stable: array order kept per env
+        import_keys_kernel<<<(C + 255) / 256, 256, 0, s>>>(M, in, m->implicit_single ? 1 : 0, keys, keys + 2 * cap);
+        size_t temp = m->import_temp.bytes();
+        NB2_CUDA_CHECK(cub::DeviceRadixSort::SortPairs(m->import_temp.get(), temp, keys, keys + cap, keys + 2 * cap, keys + 3 * cap, C, 0,
+                                                       end_bit, s));  // stable: array order kept per env
     }
-    import_scatter_kernel<<<(M.env_count + 3) / 4, 128, 0, s>>>(M, in, m->import_keys_sorted, m->import_idx_sorted);
+    import_scatter_kernel<<<(M.env_count + 3) / 4, 128, 0, s>>>(M, in, keys + cap, keys + 3 * cap);
     count_launch(2);
     NB2_CUDA_CHECK(cudaGetLastError());
     return NB2_OK;

@@ -4,11 +4,69 @@
 #include <stdint.h>
 
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/newton_b200.h"
 
 namespace nb2 {
+
+void set_error(const std::string& msg);
+
+// One device allocation, freed by the destructor.  Move-only: the model and the peer gather own their memory through these.
+class DeviceBuffer {
+  public:
+    DeviceBuffer() = default;
+    DeviceBuffer(DeviceBuffer&& o) noexcept : ptr_(std::exchange(o.ptr_, nullptr)), bytes_(std::exchange(o.bytes_, 0)) {}
+    DeviceBuffer& operator=(DeviceBuffer&& o) noexcept {
+        if (this != &o) {
+            if (ptr_) cudaFree(ptr_);
+            ptr_ = std::exchange(o.ptr_, nullptr);
+            bytes_ = std::exchange(o.bytes_, 0);
+        }
+        return *this;
+    }
+    ~DeviceBuffer() {
+        if (ptr_) cudaFree(ptr_);
+    }
+    // Replaces the buffer with `bytes` of new device memory (zero-filled when `zero`).  On failure the error is set, NB2_ERR_CUDA is
+    // returned and the buffer keeps what it held.
+    nb2_status alloc(size_t bytes, bool zero = false) {
+        void* p = nullptr;
+        cudaError_t e = cudaMalloc(&p, bytes);
+        if (e == cudaSuccess && zero) e = cudaMemset(p, 0, bytes);
+        if (e != cudaSuccess) {
+            if (p) cudaFree(p);
+            set_error(std::string("cudaMalloc / cudaMemset of ") + std::to_string(bytes) + " bytes: " + cudaGetErrorString(e));
+            return NB2_ERR_CUDA;
+        }
+        *this = DeviceBuffer();
+        ptr_ = p;
+        bytes_ = bytes;
+        return NB2_OK;
+    }
+    template <typename T = void>
+    T* get() const { return static_cast<T*>(ptr_); }
+    size_t bytes() const { return bytes_; }
+
+  private:
+    void* ptr_ = nullptr;
+    size_t bytes_ = 0;
+};
+
+// Runs an entry point on `device` and restores the caller's current device on exit (a process may drive several GPUs;
+// nb2_model_destroy is called from a garbage collector at arbitrary points).  `status` is the result of the switch.
+struct DeviceGuard {
+    int prev = -1, dev = -1;
+    cudaError_t status = cudaSuccess;
+    explicit DeviceGuard(int device) : dev(device) {
+        if (cudaGetDevice(&prev) != cudaSuccess) prev = -1;
+        if (prev != dev) status = cudaSetDevice(dev);
+    }
+    ~DeviceGuard() {
+        if (prev >= 0 && prev != dev) cudaSetDevice(prev);
+    }
+};
 
 // Number of float/int fields of one contact slot in the env-major contact blocks (DESIGN.md "contact hand-off").
 // Field f of slot s lives at cb[f * slot_total + s]: lanes read consecutive slots -> coalesced 128-byte lines.
@@ -120,30 +178,39 @@ struct nb2_model {
     int device = 0;
     nb2::DevModel dev{};
     nb2::HostTables host;
-    std::vector<void*> allocations;
+    // device memory behind the pointers of `dev` (each one is refreshed whenever its buffer is replaced)
+    nb2::DeviceBuffer env_body_start, env_joint_start, env_shape_start, env_pair_start, env_slot_start, env_art_start, global_shapes, pairs;
+    nb2::DeviceBuffer body_joint_start, body_joint_entry, joint_depth, joint_anc_mask, art_H_start, env_H_start;
+    nb2::DeviceBuffer art_batch_count, art_hb_body_start, art_hb_row_start, hb_body_col, hb_row_col, joint_desc_mask, dof_joint;
+    nb2::DeviceBuffer fs_L, contact_impulse, joint_impulse, cb;
+    nb2::DeviceBuffer env_contact_count, env_contact_offset, collide_sync, collide_tile_status;
+    nb2::DeviceBuffer collide_tile_count;  // [2][E+1]: dev.collide_tile_count, then dev.collide_tile_offset
+    nb2::DeviceBuffer dyn_pairs, env_dyn_count, filter_keys;
     int lanes_per_env = 32;  // sub-warp group width used by the fused kernels
     int featherstone_step_count = 0;
-    // scratch of nb2_contacts_import (allocated on first use, sized by the imported buffer's capacity)
+    // scratch of nb2_contacts_import (allocated on first use, sized by the imported buffer's capacity): keys, sorted keys, indices,
+    // sorted indices, capacity words each
     int import_capacity = 0;
-    int *import_keys = nullptr, *import_keys_sorted = nullptr, *import_idx = nullptr, *import_idx_sorted = nullptr;
-    void* import_temp = nullptr;
-    size_t import_temp_bytes = 0;
+    nb2::DeviceBuffer import_buf, import_temp;
     // scratch of nb2_contacts_sort (deterministic=True export order)
     int sort_capacity = 0;
-    unsigned long long *sort_keys = nullptr, *sort_keys_sorted = nullptr;
-    int *sort_idx = nullptr, *sort_idx_sorted = nullptr;
-    float* sort_stage = nullptr;  // 20 words per contact: a copy of the exported arrays to gather from
-    int* sort_rank = nullptr;     // exported index -> sorted position
-    void* sort_temp = nullptr;
-    size_t sort_temp_bytes = 0;
+    nb2::DeviceBuffer sort_keys, sort_idx;  // [2][capacity]: unsorted, then sorted
+    nb2::DeviceBuffer sort_stage;           // 20 words per contact: a copy of the exported arrays to gather from
+    nb2::DeviceBuffer sort_rank;            // exported index -> sorted position
+    nb2::DeviceBuffer sort_temp;
     // contact matching history (nb2_contacts_match): previous frame's sorted keys / world midpoints / normals / claim words
     int match_capacity = 0;
-    long long *match_new_keys = nullptr, *match_prev_keys = nullptr, *match_prev_claim = nullptr;
-    float *match_prev_pos = nullptr, *match_prev_normal = nullptr;
-    int* match_prev_count = nullptr;
-    float* match_prev_record = nullptr;      // sticky: [4][capacity] vec3 - point0, point1, offset0, offset1 of the saved frame
-    int* match_prev_was_matched = nullptr;   // contact_report: 1 where a contact of this frame kept the saved row
-    bool match_prev_has_record = false;      // the saved frame carries sticky records (the last save ran in sticky mode)
+    nb2::DeviceBuffer match_new_keys, match_prev_keys, match_prev_claim, match_prev_pos, match_prev_normal, match_prev_count;
+    nb2::DeviceBuffer match_prev_record;       // sticky: [4][capacity] vec3 - point0, point1, offset0, offset1 of the saved frame
+    nb2::DeviceBuffer match_prev_was_matched;  // contact_report: 1 where a contact of this frame kept the saved row
+    bool match_prev_has_record = false;        // the saved frame carries sticky records (the last save ran in sticky mode)
+    // Sort, import and match scratch replaced by a larger one stays allocated until the model is destroyed: a CUDA graph captured
+    // before the growth still reads it.
+    std::vector<nb2::DeviceBuffer> retired;
+    void replace_scratch(nb2::DeviceBuffer& slot, nb2::DeviceBuffer&& fresh) {
+        if (slot.get()) retired.push_back(std::move(slot));
+        slot = std::move(fresh);
+    }
     bool implicit_single = false;  // model built without begin_world(): one environment holding every entity
     bool has_convex_pairs = false;  // some pair's types have no analytic collider -> collide_kernel<L, true>
     bool has_mesh_pairs = false;    // the explicit pair list holds (mesh, infinite plane) pairs (flag NB2_PAIR_MESH_PLANE on .y)
@@ -155,7 +222,6 @@ struct nb2_model {
 };
 
 namespace nb2 {
-void set_error(const std::string& msg);
 void count_launch(int n = 1);
 nb2_status launch_collide(nb2_model* m, const float* body_q, const nb2_contacts_view* contacts, cudaStream_t s);
 nb2_status launch_broadphase(nb2_model* m, const float* body_q, cudaStream_t s);

@@ -249,83 +249,69 @@ extern "C" nb2_status nb2_contacts_match(nb2_model* m, const float* body_q, cons
         return NB2_ERR_INVALID_ARGUMENT;
     }
     cudaStream_t s = static_cast<cudaStream_t>(cuda_stream);
-    int prev = -1;
-    cudaGetDevice(&prev);
-    if (prev != m->device) cudaSetDevice(m->device);
+    DeviceGuard guard(m->device);
     const int cap = c->rigid_contact_max;
-    nb2_status st = NB2_OK;
-    do {
-        // history buffers (not capturable: the first call - or the first sticky / report call - sizes them, like the sort scratch)
-        if (cap > m->match_capacity || (sticky && !m->match_prev_record) || (report && !m->match_prev_was_matched)) {
-            for (void* p : {(void*)m->match_new_keys, (void*)m->match_prev_keys, (void*)m->match_prev_claim, (void*)m->match_prev_pos,
-                            (void*)m->match_prev_normal, (void*)m->match_prev_record, (void*)m->match_prev_was_matched})
-                if (p) cudaFree(p);
-            m->match_prev_record = nullptr;
-            m->match_prev_was_matched = nullptr;
-            m->match_prev_has_record = false;
-            void* p = nullptr;
-            const size_t rows = size_t(cap > 0 ? cap : 1);
-#define NB2_MATCH_ALLOC(field, bytes)                       \
-    if (cudaMalloc(&p, (bytes)) != cudaSuccess) {           \
-        set_error("nb2_contacts_match: out of device memory"); \
-        st = NB2_ERR_CUDA;                                  \
-        break;                                              \
-    }                                                       \
-    field = static_cast<decltype(field)>(p);
-            NB2_MATCH_ALLOC(m->match_new_keys, rows * 8)
-            NB2_MATCH_ALLOC(m->match_prev_keys, rows * 8)
-            NB2_MATCH_ALLOC(m->match_prev_claim, rows * 8)
-            NB2_MATCH_ALLOC(m->match_prev_pos, rows * 12)
-            NB2_MATCH_ALLOC(m->match_prev_normal, rows * 12)
-            if (sticky) { NB2_MATCH_ALLOC(m->match_prev_record, rows * 48) }
-            if (report) {
-                NB2_MATCH_ALLOC(m->match_prev_was_matched, rows * 4)
-                cudaMemsetAsync(m->match_prev_was_matched, 0, rows * 4, s);
-            }
-#undef NB2_MATCH_ALLOC
-            if (!m->match_prev_count) {
-                if (cudaMalloc(&p, sizeof(int)) != cudaSuccess) {
-                    st = NB2_ERR_CUDA;
-                    break;
-                }
-                m->match_prev_count = static_cast<int*>(p);
-            }
-            cudaMemsetAsync(m->match_prev_count, 0, sizeof(int), s);
-            m->match_capacity = cap;
+    // history buffers (not capturable: the first call - or the first sticky / report call - sizes them, like the sort scratch)
+    if (cap > m->match_capacity || (sticky && !m->match_prev_record.get()) || (report && !m->match_prev_was_matched.get())) {
+        const size_t rows = size_t(cap > 0 ? cap : 1);
+        DeviceBuffer new_keys, prev_keys, prev_claim, prev_pos, prev_normal, prev_record, prev_was_matched, prev_count;
+        if (new_keys.alloc(rows * 8) || prev_keys.alloc(rows * 8) || prev_claim.alloc(rows * 8) || prev_pos.alloc(rows * 12) ||
+            prev_normal.alloc(rows * 12) || (sticky && prev_record.alloc(rows * 48)) || (report && prev_was_matched.alloc(rows * 4)) ||
+            (!m->match_prev_count.get() && prev_count.alloc(sizeof(int)))) {
+            set_error("nb2_contacts_match: out of device memory");
+            return NB2_ERR_CUDA;
         }
-        if (opt->reset_all) cudaMemsetAsync(m->match_prev_count, 0, sizeof(int), s);
-        if (cap > 0) {
-            const int blocks = (cap + 255) / 256;
-            // a history that was saved without sticky records / report flags keeps working: those buffers are only used when present
-            match_keys_kernel<<<blocks, 256, 0, s>>>(*c, m->match_new_keys);
-            match_contacts_kernel<<<blocks, 256, 0, s>>>(m->dev.d, *c, body_q, m->match_new_keys, m->match_prev_keys, m->match_prev_pos,
-                                                         m->match_prev_normal, m->match_prev_count, m->match_prev_claim, opt->reset_world_mask,
-                                                         opt->pos_threshold * opt->pos_threshold, opt->normal_dot_threshold, match_index);
-            match_resolve_kernel<<<blocks, 256, 0, s>>>(*c, m->match_new_keys, m->match_prev_claim, match_index, m->match_prev_was_matched);
-            int launched = 4;
-            if (sticky && m->match_prev_has_record) {
-                match_replay_kernel<<<blocks, 256, 0, s>>>(m->dev.d, *c, body_q, match_index, m->match_prev_record, m->match_prev_normal, m->match_capacity);
-                ++launched;
-            }
-            if (report) {
-                match_report_kernel<<<1, 1024, 0, s>>>(m->dev.d, *c, match_index, m->match_prev_keys, m->match_prev_count, m->match_prev_was_matched,
-                                                       opt->reset_world_mask, opt->new_indices, opt->new_count, opt->broken_indices, opt->broken_count);
-                ++launched;
-            }
-            match_save_kernel<<<blocks, 256, 0, s>>>(m->dev.d, *c, body_q, m->match_new_keys, m->match_prev_keys, m->match_prev_pos,
-                                                     m->match_prev_normal, m->match_prev_claim, m->match_prev_count, m->match_prev_was_matched,
-                                                     sticky ? m->match_prev_record : nullptr, m->match_capacity);
-            m->match_prev_has_record = sticky;
-            count_launch(launched);
-            if (cudaGetLastError() != cudaSuccess) {
-                set_error("nb2_contacts_match: kernel launch failed");
-                st = NB2_ERR_CUDA;
-            }
-        } else if (report) {
-            cudaMemsetAsync(opt->new_count, 0, sizeof(int), s);
-            cudaMemsetAsync(opt->broken_count, 0, sizeof(int), s);
+        m->replace_scratch(m->match_new_keys, std::move(new_keys));
+        m->replace_scratch(m->match_prev_keys, std::move(prev_keys));
+        m->replace_scratch(m->match_prev_claim, std::move(prev_claim));
+        m->replace_scratch(m->match_prev_pos, std::move(prev_pos));
+        m->replace_scratch(m->match_prev_normal, std::move(prev_normal));
+        m->replace_scratch(m->match_prev_record, std::move(prev_record));
+        m->replace_scratch(m->match_prev_was_matched, std::move(prev_was_matched));
+        if (prev_count.get()) m->match_prev_count = std::move(prev_count);
+        if (report) cudaMemsetAsync(m->match_prev_was_matched.get(), 0, rows * 4, s);
+        cudaMemsetAsync(m->match_prev_count.get(), 0, sizeof(int), s);
+        m->match_prev_has_record = false;
+        m->match_capacity = cap;
+    }
+    long long* new_keys = m->match_new_keys.get<long long>();
+    long long* prev_keys = m->match_prev_keys.get<long long>();
+    long long* prev_claim = m->match_prev_claim.get<long long>();
+    float* prev_pos = m->match_prev_pos.get<float>();
+    float* prev_normal = m->match_prev_normal.get<float>();
+    float* prev_record = m->match_prev_record.get<float>();
+    int* prev_count = m->match_prev_count.get<int>();
+    int* prev_was_matched = m->match_prev_was_matched.get<int>();
+    if (opt->reset_all) cudaMemsetAsync(prev_count, 0, sizeof(int), s);
+    if (cap > 0) {
+        const int blocks = (cap + 255) / 256;
+        // a history that was saved without sticky records / report flags keeps working: those buffers are only used when present
+        match_keys_kernel<<<blocks, 256, 0, s>>>(*c, new_keys);
+        match_contacts_kernel<<<blocks, 256, 0, s>>>(m->dev.d, *c, body_q, new_keys, prev_keys, prev_pos, prev_normal, prev_count, prev_claim,
+                                                     opt->reset_world_mask, opt->pos_threshold * opt->pos_threshold,
+                                                     opt->normal_dot_threshold, match_index);
+        match_resolve_kernel<<<blocks, 256, 0, s>>>(*c, new_keys, prev_claim, match_index, prev_was_matched);
+        int launched = 4;
+        if (sticky && m->match_prev_has_record) {
+            match_replay_kernel<<<blocks, 256, 0, s>>>(m->dev.d, *c, body_q, match_index, prev_record, prev_normal, m->match_capacity);
+            ++launched;
         }
-    } while (0);
-    if (prev >= 0 && prev != m->device) cudaSetDevice(prev);
-    return st;
+        if (report) {
+            match_report_kernel<<<1, 1024, 0, s>>>(m->dev.d, *c, match_index, prev_keys, prev_count, prev_was_matched, opt->reset_world_mask,
+                                                   opt->new_indices, opt->new_count, opt->broken_indices, opt->broken_count);
+            ++launched;
+        }
+        match_save_kernel<<<blocks, 256, 0, s>>>(m->dev.d, *c, body_q, new_keys, prev_keys, prev_pos, prev_normal, prev_claim, prev_count,
+                                                 prev_was_matched, sticky ? prev_record : nullptr, m->match_capacity);
+        m->match_prev_has_record = sticky;
+        count_launch(launched);
+        if (cudaGetLastError() != cudaSuccess) {
+            set_error("nb2_contacts_match: kernel launch failed");
+            return NB2_ERR_CUDA;
+        }
+    } else if (report) {
+        cudaMemsetAsync(opt->new_count, 0, sizeof(int), s);
+        cudaMemsetAsync(opt->broken_count, 0, sizeof(int), s);
+    }
+    return NB2_OK;
 }

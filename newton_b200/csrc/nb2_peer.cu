@@ -11,20 +11,28 @@
 
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 
 #include "nb2_internal.cuh"
 
 struct nb2_peer_gather {
     int device = 0, rank = 0, world = 1;
     size_t bytes_per_rank = 0;
-    char* recv = nullptr;      // [2 slots][world][bytes_per_rank]
-    int* flags = nullptr;      // [2 slots][world] sequence numbers
+    nb2::DeviceBuffer recv;        // [2 slots][world][bytes_per_rank]
+    nb2::DeviceBuffer flags;       // [2 slots][world] int sequence numbers
     std::vector<char*> peer_recv;  // peer-mapped addresses (own rank: the local pointers)
     std::vector<int*> peer_flags;
-    int** d_peer_flags = nullptr;  // device copy of peer_flags for the signal kernel
-    bool memops = false;           // publish with cuStreamWriteValue32 instead of the one-thread signal kernel
+    nb2::DeviceBuffer d_peer_flags;  // device copy of peer_flags for the signal kernel
+    bool memops = false;             // publish with cuStreamWriteValue32 instead of the one-thread signal kernel
     CUresult (*wait32)(CUstream, CUdeviceptr, cuuint32_t, unsigned int) = nullptr;
     CUresult (*write32)(CUstream, CUdeviceptr, cuuint32_t, unsigned int) = nullptr;
+    ~nb2_peer_gather() {  // unmaps the peers' buffers; the own buffers free themselves
+        for (size_t p = 0; p < peer_recv.size(); ++p) {
+            if (int(p) == rank) continue;
+            if (peer_recv[p]) cudaIpcCloseMemHandle(peer_recv[p]);
+            if (peer_flags[p]) cudaIpcCloseMemHandle(peer_flags[p]);
+        }
+    }
 };
 
 namespace nb2 {
@@ -58,26 +66,24 @@ nb2_status nb2_peer_gather_create(int32_t device, int32_t rank, int32_t world_si
         return NB2_ERR_INVALID_ARGUMENT;
     }
     *out = nullptr;
-    int prev = -1;
-    cudaGetDevice(&prev);
-    NB2_CUDA_CHECK(cudaSetDevice(device));
-    nb2_peer_gather* g = new nb2_peer_gather();
+    DeviceGuard guard(device);
+    if (guard.status != cudaSuccess) {
+        set_error(std::string("cudaSetDevice(device): ") + cudaGetErrorString(guard.status));
+        return NB2_ERR_CUDA;
+    }
+    std::unique_ptr<nb2_peer_gather> g(new nb2_peer_gather());
     g->device = device;
     g->rank = rank;
     g->world = world_size;
     g->bytes_per_rank = (bytes_per_rank + 15) & ~size_t(15);
-    void* p = nullptr;
-    NB2_CUDA_CHECK(cudaMalloc(&p, 2 * size_t(world_size) * g->bytes_per_rank));
-    g->recv = static_cast<char*>(p);
-    NB2_CUDA_CHECK(cudaMalloc(&p, 2 * size_t(world_size) * sizeof(int)));
-    g->flags = static_cast<int*>(p);
-    NB2_CUDA_CHECK(cudaMemset(g->flags, 0, 2 * size_t(world_size) * sizeof(int)));
-    NB2_CUDA_CHECK(cudaMalloc(&p, size_t(world_size) * sizeof(int*)));
-    g->d_peer_flags = static_cast<int**>(p);
+    nb2_status st;
+    if ((st = g->recv.alloc(2 * size_t(world_size) * g->bytes_per_rank))) return st;
+    if ((st = g->flags.alloc(2 * size_t(world_size) * sizeof(int), true))) return st;
+    if ((st = g->d_peer_flags.alloc(size_t(world_size) * sizeof(int*)))) return st;
     g->peer_recv.assign(size_t(world_size), nullptr);
     g->peer_flags.assign(size_t(world_size), nullptr);
-    g->peer_recv[rank] = g->recv;
-    g->peer_flags[rank] = g->flags;
+    g->peer_recv[rank] = g->recv.get<char>();
+    g->peer_flags[rank] = g->flags.get<int>();
     cudaDriverEntryPointQueryResult q;
     void* fn = nullptr;
     if (cudaGetDriverEntryPoint("cuStreamWaitValue32", &fn, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
@@ -87,13 +93,12 @@ nb2_status nb2_peer_gather_create(int32_t device, int32_t rank, int32_t world_si
         g->write32 = reinterpret_cast<decltype(g->write32)>(fn);
     cudaGetLastError();
     if (const char* v = std::getenv("NB2_PEER_MEMOPS")) g->memops = std::atoi(v) != 0 && g->write32;
-    if (prev >= 0 && prev != device) cudaSetDevice(prev);
-    *out = g;
+    *out = g.release();
     return NB2_OK;
 }
 
 void* nb2_peer_gather_buffer(nb2_peer_gather* g, int32_t slot) {
-    return g ? g->recv + size_t(slot & 1) * size_t(g->world) * g->bytes_per_rank : nullptr;
+    return g ? g->recv.get<char>() + size_t(slot & 1) * size_t(g->world) * g->bytes_per_rank : nullptr;
 }
 size_t nb2_peer_gather_stride(const nb2_peer_gather* g) { return g ? g->bytes_per_rank : 0; }
 
@@ -103,8 +108,8 @@ nb2_status nb2_peer_gather_export(nb2_peer_gather* g, void* handle_out) {
         return NB2_ERR_INVALID_ARGUMENT;
     }
     cudaIpcMemHandle_t h[2];
-    NB2_CUDA_CHECK(cudaIpcGetMemHandle(&h[0], g->recv));
-    NB2_CUDA_CHECK(cudaIpcGetMemHandle(&h[1], g->flags));
+    NB2_CUDA_CHECK(cudaIpcGetMemHandle(&h[0], g->recv.get()));
+    NB2_CUDA_CHECK(cudaIpcGetMemHandle(&h[1], g->flags.get()));
     std::memcpy(handle_out, h, sizeof(h));
     return NB2_OK;
 }
@@ -116,9 +121,11 @@ nb2_status nb2_peer_gather_connect(nb2_peer_gather* g, const void* all_handles) 
         set_error("nb2_peer_gather_connect: NULL argument");
         return NB2_ERR_INVALID_ARGUMENT;
     }
-    int prev = -1;
-    cudaGetDevice(&prev);
-    NB2_CUDA_CHECK(cudaSetDevice(g->device));
+    DeviceGuard guard(g->device);
+    if (guard.status != cudaSuccess) {
+        set_error(std::string("cudaSetDevice(g->device): ") + cudaGetErrorString(guard.status));
+        return NB2_ERR_CUDA;
+    }
     const char* base = static_cast<const char*>(all_handles);
     for (int p = 0; p < g->world; ++p) {
         if (p == g->rank) continue;
@@ -131,8 +138,7 @@ nb2_status nb2_peer_gather_connect(nb2_peer_gather* g, const void* all_handles) 
         g->peer_recv[p] = static_cast<char*>(a);
         g->peer_flags[p] = static_cast<int*>(b);
     }
-    NB2_CUDA_CHECK(cudaMemcpy(g->d_peer_flags, g->peer_flags.data(), size_t(g->world) * sizeof(int*), cudaMemcpyHostToDevice));
-    if (prev >= 0 && prev != g->device) cudaSetDevice(prev);
+    NB2_CUDA_CHECK(cudaMemcpy(g->d_peer_flags.get(), g->peer_flags.data(), size_t(g->world) * sizeof(int*), cudaMemcpyHostToDevice));
     return NB2_OK;
 }
 
@@ -163,7 +169,7 @@ nb2_status nb2_peer_gather_push(nb2_peer_gather* g, const void* src, size_t byte
             }
         }
     } else {
-        peer_signal_kernel<<<1, 32, 0, s>>>(g->d_peer_flags, g->world, flag_index, sequence);
+        peer_signal_kernel<<<1, 32, 0, s>>>(g->d_peer_flags.get<int*>(), g->world, flag_index, sequence);
         count_launch();
         NB2_CUDA_CHECK(cudaGetLastError());
     }
@@ -177,7 +183,7 @@ nb2_status nb2_peer_gather_wait(nb2_peer_gather* g, int32_t sequence, void* cuda
         return NB2_ERR_INVALID_ARGUMENT;
     }
     cudaStream_t s = static_cast<cudaStream_t>(cuda_stream);
-    const int* f = g->flags + (sequence & 1) * g->world;
+    const int* f = g->flags.get<int>() + (sequence & 1) * g->world;
     if (g->wait32) {
         for (int p = 0; p < g->world; ++p) {
             const CUresult r = g->wait32(s, reinterpret_cast<CUdeviceptr>(f + p), cuuint32_t(sequence), CU_STREAM_WAIT_VALUE_GEQ);
@@ -196,18 +202,7 @@ nb2_status nb2_peer_gather_wait(nb2_peer_gather* g, int32_t sequence, void* cuda
 
 void nb2_peer_gather_destroy(nb2_peer_gather* g) {
     if (!g) return;
-    int prev = -1;
-    cudaGetDevice(&prev);
-    cudaSetDevice(g->device);
-    for (int p = 0; p < g->world; ++p) {
-        if (p == g->rank) continue;
-        if (g->peer_recv[p]) cudaIpcCloseMemHandle(g->peer_recv[p]);
-        if (g->peer_flags[p]) cudaIpcCloseMemHandle(g->peer_flags[p]);
-    }
-    cudaFree(g->recv);
-    cudaFree(g->flags);
-    cudaFree(g->d_peer_flags);
-    if (prev >= 0 && prev != g->device) cudaSetDevice(prev);
+    DeviceGuard guard(g->device);
     delete g;
 }
 
