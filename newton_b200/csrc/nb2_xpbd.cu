@@ -27,8 +27,10 @@ namespace nb2 {
 enum { JT_PRISMATIC = 0, JT_REVOLUTE = 1, JT_BALL = 2, JT_FIXED = 3, JT_FREE = 4, JT_DISTANCE = 5, JT_D6 = 6, JT_ROD = 7 };
 enum { BODY_KINEMATIC = 2 };
 
-// shared-memory body record (floats): odd stride -> consecutive bodies hit different banks
-enum { BR_Q = 0, BR_QD = 7, BR_COM = 13, BR_INVM = 16, BR_INVI = 17, BR_I = 26, BR_SIZE = 35 };
+// shared-memory body record (floats): odd stride -> consecutive bodies hit different banks.  BR_WCOM is the world centre of mass
+// xpoint(pose, com) of the pose in BR_Q, formed with the very same expression wherever the pose is written (integrate, apply_delta),
+// so that the contact and joint rows and the next apply_delta read it instead of rotating com again.  Word 38 is padding.
+enum { BR_Q = 0, BR_QD = 7, BR_COM = 13, BR_INVM = 16, BR_INVI = 17, BR_I = 26, BR_WCOM = 35, BR_SIZE = 39 };
 enum { DR_SIZE = 13 };  // delta record: lin_a, ang_a, lin_b, ang_b, active
 enum { XF_JOINT_CACHE = 1, XF_TMA = 2, XF_PHASE_SYNC = 4, XF_PHASE_SYNC_FINE = 8 };  // kernel flags
 // per-contact constants of the Jacobi loop, staged once per substep: point0, point1, normal, margin0 + margin1, the three friction
@@ -51,9 +53,34 @@ enum { CC_P0 = 0, CC_P1 = 3, CC_N = 6, CC_MSUM = 9, CC_MU = 10, CC_MUT = 11, CC_
 #define NB2_ROW_UNROLL _Pragma("unroll 1")
 #endif
 
+// Per-phase timing, diagnostic build only (-DNB2_XPBD_PHASE_CLOCKS, scripts/xpbd_phase_breakdown.py).  Lane 0 of every warp of
+// xpbd_step_kernel stores clock64() at the phase boundaries of the substep into one record per warp: [0] kernel start, [1] start of
+// the Jacobi loop, then per iteration five words (after the iteration barrier, after the contact rows, after the contact apply,
+// after the joint rows, after the joint apply), then the end of the loop and the end of the kernel.  Plain stores: every launch
+// overwrites the records its warps reach, nothing waits on them.  The product build compiles none of this.
+#ifdef NB2_XPBD_PHASE_CLOCKS
+enum { PC_MAX_WARPS = 4096, PC_MAX_IT = 16, PC_LOOP_END = 2 + 5 * PC_MAX_IT, PC_END = PC_LOOP_END + 1, PC_WORDS = PC_END + 1 };
+__device__ long long nb2_xpbd_phase_clk[PC_MAX_WARPS * PC_WORDS];
+#define NB2_PHASE_CLOCK(word)                                         \
+    do {                                                              \
+        if (pc_rec != nullptr && lane == 0) pc_rec[word] = clock64(); \
+    } while (0)
+#define NB2_PHASE_CLOCK_IT(it, k)                      \
+    do {                                               \
+        if ((it) < PC_MAX_IT) NB2_PHASE_CLOCK(2 + 5 * (it) + (k)); \
+    } while (0)
+#else
+#define NB2_PHASE_CLOCK(word) \
+    do {                      \
+    } while (0)
+#define NB2_PHASE_CLOCK_IT(it, k) \
+    do {                          \
+    } while (0)
+#endif
+
 struct BodyView {
     Xf X;
-    V3 com;
+    V3 wcom;  // xpoint(X, com)
     float inv_m;
     const float* rec;  // shared-memory record (inverse inertia is read from it on demand); nullptr = the static world
     V3 v, w;
@@ -64,7 +91,7 @@ NB2_DEV BodyView load_body(const float* rec) {
     b.X = ldx(rec + BR_Q);
     b.v = ld3(rec + BR_QD);
     b.w = ld3(rec + BR_QD + 3);
-    b.com = ld3(rec + BR_COM);
+    b.wcom = ld3(rec + BR_WCOM);
     b.inv_m = rec[BR_INVM];
     b.rec = rec;
     return b;
@@ -228,8 +255,9 @@ NB2_DEV bool solve_joint(const nb2_model_desc& d, const nb2_control_view& ctl, c
     const int axis_start = jc ? jc_int(jc, JC_AXIS) : d.joint_qd_start[j];
     const int target_start = jc ? jc_int(jc, JC_TARGET) : d.joint_target_q_start[j];
     const int lin_count = (hdr >> 8) & 15, ang_count = (hdr >> 12) & 15;
-    const V3 wcom_p = xpoint(pose_p, bp.com);
-    const V3 wcom_c = xpoint(pose_c, bc.com);
+    // xpoint(pose, com) of both bodies; the static world's centre of mass is the zero vector
+    const V3 wcom_p = id_p >= 0 ? bp.wcom : xpoint(pose_p, V3());
+    const V3 wcom_c = bc.wcom;
     const V3 vel_p = bp.v, omega_p = bp.w, vel_c = bc.v, omega_c = bc.w;
 
     if (type == JT_DISTANCE) {
@@ -262,7 +290,8 @@ NB2_DEV bool solve_joint(const nb2_model_desc& d, const nb2_control_view& ctl, c
             ang_dc += ac * (dl * P.joint_angular_relaxation);
         }
     } else {
-        const AxisSetup s = gather_axes(d, ctl, axis_start, target_start, 0, lin_count);
+        // without linear dofs gather_axes returns AxisSetup() (its axis loop does not run, no division is taken): skip its loads
+        const AxisSetup s = lin_count == 0 ? AxisSetup() : gather_axes(d, ctl, axis_start, target_start, 0, lin_count);
         V3 proj = rel_p;
 #pragma unroll
         for (int dim = 0; dim < 3; ++dim) {
@@ -477,9 +506,10 @@ NB2_HELPER void apply_delta(float* rec, V3 dlin, V3 dang, float inv_weight, bool
                         q0.w * hh.z + hh.x * q0.y - q0.x * hh.y, -hh.x * q0.x - hh.y * q0.y - hh.z * q0.z));
     q1 = qunit(q1);
     const V3 com = ld3(rec + BR_COM);
-    const V3 x_com = p0 + qrot(q0, com);
+    const V3 x_com = ld3(rec + BR_WCOM);  // p0 + qrot(q0, com)
+    const V3 com1 = qrot(q1, com);
     V3 p1 = x_com + dp * dt;
-    p1 -= qrot(q1, com);
+    p1 -= com1;
     V3 v1 = v0 + dp, w1 = w0 + dw1;
     // len(v) < 1e-4f without the square root: sqrtf is correctly rounded and monotonic, and 0x1.5798ecp-27f (1e-4f * 1e-4f rounded)
     // is the smallest float whose square root rounds to 1e-4f or more, so the two tests agree for every input, NaN included
@@ -487,6 +517,7 @@ NB2_HELPER void apply_delta(float* rec, V3 dlin, V3 dang, float inv_weight, bool
     if (len2(w1) < 0x1.5798ecp-27f) w1 = V3();
     st3(rec + BR_Q, p1);
     rec[BR_Q + 3] = q1.x; rec[BR_Q + 4] = q1.y; rec[BR_Q + 5] = q1.z; rec[BR_Q + 6] = q1.w;
+    st3(rec + BR_WCOM, p1 + com1);  // xpoint((p1, q1), com)
     st3(rec + BR_QD, v1);
     st3(rec + BR_QD + 3, w1);
 }
@@ -574,6 +605,11 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
     const int slot = warp * G + grp;  // environment slot inside the CTA
     const int env0 = blockIdx.x * NE;
     if (env0 >= M.env_count) return;  // padding CTA of the NB2_XPBD_MIN_GRID experiment (whole CTA, before any barrier)
+#ifdef NB2_XPBD_PHASE_CLOCKS
+    const int pc_warp = blockIdx.x * WARPS + warp;
+    long long* pc_rec = pc_warp < PC_MAX_WARPS ? nb2_xpbd_phase_clk + size_t(pc_warp) * PC_WORDS : nullptr;
+#endif
+    NB2_PHASE_CLOCK(0);
     const int env = env0 + slot;
     const bool live = env < M.env_count;
     const nb2_model_desc& d = M.d;
@@ -746,7 +782,10 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
                 else { f0 -= ld3(r + 0); t0 -= ld3(r + 3); }
             }
         }
-        if ((d.body_flags[gb] & BODY_KINEMATIC) != 0) continue;  // kinematic bodies pass through (solver.py:132-139)
+        if ((d.body_flags[gb] & BODY_KINEMATIC) != 0) {  // kinematic bodies pass through (solver.py:132-139)
+            st3(rec + BR_WCOM, xpoint(ldx(rec + BR_Q), ld3(rec + BR_COM)));
+            continue;
+        }
         const V3 x0 = ld3(rec + BR_Q);
         const Q4 r0(rec[BR_Q + 3], rec[BR_Q + 4], rec[BR_Q + 5], rec[BR_Q + 6]);
         const V3 v0 = ld3(rec + BR_QD), w0 = ld3(rec + BR_QD + 3);
@@ -765,8 +804,10 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
         V3 w1 = qrot(r0, wb + mv(inv_inertia, tb) * dt);
         const Q4 r1 = qunit(qadd(r0, qscale(qscale(qmul(Q4(w1.x, w1.y, w1.z, 0.0f), r0), 0.5f), dt)));
         w1 *= 1.0f - P.angular_damping * dt;
-        st3(rec + BR_Q, x1 - qrot(r1, com));
+        const V3 com1 = qrot(r1, com), x1_origin = x1 - com1;
+        st3(rec + BR_Q, x1_origin);
         rec[BR_Q + 3] = r1.x; rec[BR_Q + 4] = r1.y; rec[BR_Q + 5] = r1.z; rec[BR_Q + 6] = r1.w;
+        st3(rec + BR_WCOM, x1_origin + com1);  // xpoint((x1_origin, r1), com)
         st3(rec + BR_QD, v1);
         st3(rec + BR_QD + 3, w1);
     }
@@ -775,11 +816,13 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
     const size_t T = size_t(M.slot_total);
     const float* cb = M.cb;
     const float lin_alpha_dt = P.joint_linear_compliance / dt, ang_alpha_dt = P.joint_angular_compliance / dt;
+    NB2_PHASE_CLOCK(1);
     for (int it = 0; it < P.iterations; ++it) {
         // CTA barriers are not needed for correctness (a warp owns its environments); they keep the CTA's warps on the same
         // stretch of code so that the instruction stream is fetched once per CTA (see the kernel comment)
         const bool sync_it = (flags & XF_PHASE_SYNC) && WARPS > 1, sync_fine = (flags & XF_PHASE_SYNC_FINE) && WARPS > 1;
         if (sync_it) __syncthreads();
+        NB2_PHASE_CLOCK_IT(it, 0);
         if (use_contacts) {
             // ---- [iteration] solve_body_contact_positions (kernels.py:2164-2399)
             for (int c = l; c < nc; c += L) {
@@ -807,7 +850,7 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
                         active = 1.0f;
                         const float mu = cached ? cc[CC_MU] : cb[CF_MU * T + s], mu_t = cached ? cc[CC_MUT] : cb[CF_MU_TORSIONAL * T + s],
                                     mu_r = cached ? cc[CC_MUR] : cb[CF_MU_ROLLING * T + s];
-                        const V3 wcom_a = ba >= 0 ? xpoint(A.X, A.com) : V3(), wcom_b = bb >= 0 ? xpoint(B.X, B.com) : V3();
+                        const V3 wcom_a = ba >= 0 ? A.wcom : V3(), wcom_b = bb >= 0 ? B.wcom : V3();
                         V3 r_a = bx_a - wcom_a, r_b = bx_b - wcom_b;
                         V3 ang_a, ang_b;
                         if (need_a) ang_a = -cross(r_a, n);
@@ -883,6 +926,7 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
                 store_deltas(drec + c * DR_SIZE, dl, active);
             }
             __syncwarp();
+            NB2_PHASE_CLOCK_IT(it, 1);
             if (sync_fine) __syncthreads();
             // ---- [iteration] ordered per-body sum (contact order; side A before side B) + weighted apply
             for (int b = l; b < nb; b += L) {
@@ -936,6 +980,7 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
                 __syncwarp();
             }
         }
+        NB2_PHASE_CLOCK_IT(it, 2);
         if (d.joint_count > 0) {
             if (sync_fine) __syncthreads();
             // ---- [iteration] solve_body_joints (kernels.py:1513-2044) + ordered per-body apply
@@ -952,6 +997,7 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
                 }
             }
             __syncwarp();
+            NB2_PHASE_CLOCK_IT(it, 3);
             if (sync_fine) __syncthreads();
             for (int b = l; b < nb; b += L) {
                 const int gb = b0 + b;
@@ -967,7 +1013,9 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
             }
             __syncwarp();
         }
+        NB2_PHASE_CLOCK_IT(it, 4);
     }
+    NB2_PHASE_CLOCK(PC_LOOP_END);
     if (EX) {
         // ---- State.body_parent_f (convert_joint_impulse_to_parent_f, kernels.py:2497-2544): joints in index order per child ----
         if (sout.body_parent_f != nullptr) {
@@ -1112,6 +1160,7 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
             bulk_s2g(sout.body_qd + 6 * size_t(cb0), stage + ST_QD * cnb, unsigned(cnb) * 24u);
             bulk_commit_and_drain();  // shared memory must stay alive until the TMA unit has read it
         }
+        NB2_PHASE_CLOCK(PC_END);
         return;
     }
     for (int b = l; b < nb; b += L) {
@@ -1122,6 +1171,7 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
 #pragma unroll
         for (int k = 0; k < 6; ++k) sout.body_qd[6 * gb + k] = rec[BR_QD + k];
     }
+    NB2_PHASE_CLOCK(PC_END);
 }
 
 // SolverXPBD.update_contacts (solver_xpbd.py:864-925): force[i] = weighted impulse of exported contact i / dt
@@ -1323,3 +1373,15 @@ nb2_status launch_integrate_bodies(nb2_model* m, const nb2_state_view& in, const
 }
 
 }  // namespace nb2
+
+#ifdef NB2_XPBD_PHASE_CLOCKS
+// Read back the per-warp phase clocks of the last xpbd_step launch on the current device (layout above the kernel).
+extern "C" void nb2_xpbd_phase_clock_shape(int* max_warps, int* max_iterations, int* words_per_warp) {
+    *max_warps = nb2::PC_MAX_WARPS;
+    *max_iterations = nb2::PC_MAX_IT;
+    *words_per_warp = nb2::PC_WORDS;
+}
+extern "C" int nb2_xpbd_phase_clocks(long long* out) {
+    return cudaMemcpyFromSymbol(out, nb2::nb2_xpbd_phase_clk, sizeof(nb2::nb2_xpbd_phase_clk)) == cudaSuccess ? 0 : -1;
+}
+#endif
