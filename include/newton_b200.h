@@ -488,6 +488,38 @@ nb2_status nb2_intersect_ray(const nb2_raycast_view* view, int32_t ray_count, co
                              const int32_t* ray_worlds, int32_t enable_global_world, float* out_dist, int32_t* out_shape_id,
                              float* out_normal, void* cuda_stream);
 
+/* Tiled depth camera (reference SensorTiledCamera.update, sensors/warp_raytrace/render.py:86-345), one thread per pixel of every
+ * (world, camera) image.  Pixel (w, c, y, x): o = transform_point(T[c, w], rays[c, y, x, 0]), d = transform_vector(T[c, w],
+ * rays[c, y, x, 1]) (d is not renormalised: depth is the ray parameter t).  dot(d, d) <= 1e-12 clears the pixel.  Otherwise the
+ * closest hit over world w's group, then the global group when NB2_CAMERA_GLOBAL_WORLD is set, starting from max_distance:
+ * the walk of nb2_intersect_ray, except that only MESH shapes take the mesh test (CONVEX_MESH shapes are never hit, as in the
+ * reference camera) and NB2_CAMERA_BACKFACE_CULLING rejects planes seen from below and meshes whose closest triangle faces
+ * away from the ray.  A hit writes depth t, forward depth t * dot(d, normalize(transform_vector(T, (0, 0, -1)))), the world
+ * normal and the shape id; a miss writes the clear values.  Outputs are [world_count, camera_count, height, width] (normal
+ * x 3); any may be NULL and only those given are written.  Reads the shape table of the last nb2_raycast_refit and writes
+ * nothing when the view has no enabled shape.  A pixel total past INT32_MAX is refused with NB2_ERR_CAPACITY. */
+enum { NB2_CAMERA_GLOBAL_WORLD = 1, NB2_CAMERA_BACKFACE_CULLING = 2 };
+
+typedef struct nb2_camera_desc {
+    int32_t world_count;             /* must equal the view's world_count */
+    int32_t camera_count;
+    int32_t width;
+    int32_t height;
+    const float* camera_rays;        /* [camera_count, height, width, 2, 3] camera-space origin, direction */
+    const float* camera_transforms;  /* [camera_count, world_count, 7] camera-to-world (p, q xyzw) */
+    float max_distance;
+    int32_t flags;                   /* NB2_CAMERA_* */
+    float* depth;                    /* [W, C, H, Wd] or NULL */
+    float* forward_depth;            /* [W, C, H, Wd] or NULL */
+    uint32_t* shape_index;           /* [W, C, H, Wd] or NULL */
+    float* normal;                   /* [W, C, H, Wd, 3] or NULL */
+    float clear_depth;               /* depth and forward depth of a miss */
+    uint32_t clear_shape_index;
+    float clear_normal[3];
+} nb2_camera_desc;
+
+nb2_status nb2_camera_render(const nb2_raycast_view* view, const nb2_camera_desc* camera, void* cuda_stream);
+
 /* --- actuators (reference newton.actuators, actuators/) --------------------------------------------------------------------
  * One thread per actuator of one group: delayed or current targets -> PD / PID -> clamp chain -> out[idx] = out[idx] + f ->
  * delay buffer and PID state of the next state.  Index arrays are int32 (the reference's uint32 values).  The host

@@ -236,6 +236,16 @@ class RaycastView(C.Structure):
 
 
 RAYCAST_MAX_DEPTH = 48  # NB2_RAYCAST_MAX_DEPTH
+CAMERA_GLOBAL_WORLD, CAMERA_BACKFACE_CULLING = 1, 2  # NB2_CAMERA_*
+
+
+class CameraDesc(C.Structure):
+    """``nb2_camera_desc``"""
+
+    _fields_ = [("world_count", C.c_int32), ("camera_count", C.c_int32), ("width", C.c_int32), ("height", C.c_int32),
+                ("camera_rays", C.c_void_p), ("camera_transforms", C.c_void_p), ("max_distance", C.c_float), ("flags", C.c_int32),
+                ("depth", C.c_void_p), ("forward_depth", C.c_void_p), ("shape_index", C.c_void_p), ("normal", C.c_void_p),
+                ("clear_depth", C.c_float), ("clear_shape_index", C.c_uint32), ("clear_normal", C.c_float * 3)]
 
 
 ACT_PD, ACT_PID = 0, 1  # NB2_ACT_*

@@ -939,6 +939,35 @@ nb2_status nb2_intersect_ray(const nb2_raycast_view* view, int32_t ray_count, co
                                 out_normal, static_cast<cudaStream_t>(cuda_stream));
 }
 
+nb2_status nb2_camera_render(const nb2_raycast_view* view, const nb2_camera_desc* camera, void* cuda_stream) {
+    if (!raycast_view_valid(view, "nb2_camera_render")) return NB2_ERR_INVALID_ARGUMENT;
+    if (!camera) {
+        set_error("nb2_camera_render: NULL camera descriptor");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    const nb2_camera_desc& c = *camera;
+    if (c.world_count != view->world_count || c.camera_count < 0 || c.width < 0 || c.height < 0) {
+        set_error("nb2_camera_render: world_count differs from the view's, or a negative camera_count, width or height");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    if ((c.flags & ~(NB2_CAMERA_GLOBAL_WORLD | NB2_CAMERA_BACKFACE_CULLING)) != 0) {
+        set_error("nb2_camera_render: unknown flag bits");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    const int64_t pixels = (int64_t)c.world_count * c.camera_count * c.width * c.height;
+    if (pixels > INT32_MAX) {
+        set_error("nb2_camera_render: " + std::to_string(pixels) + " pixels; at most 2^31 - 1 per call");
+        return NB2_ERR_CAPACITY;
+    }
+    const bool any_output = c.depth || c.forward_depth || c.shape_index || c.normal;
+    if (pixels == 0 || !any_output) return NB2_OK;
+    if (!c.camera_rays || !c.camera_transforms) {
+        set_error("nb2_camera_render: NULL camera_rays or camera_transforms with an output requested");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    return launch_camera_render(*view, c, static_cast<cudaStream_t>(cuda_stream));
+}
+
 nb2_status nb2_ik_solve(const nb2_ik_desc* desc, const float* joint_q_in, float* joint_q, float* joint_q_out, float* residuals,
                         float* costs, float* lambda_values, float* jacobian, int32_t iterations, float step_size, int32_t write_lambda,
                         uint32_t* seed_state, void* cuda_stream) {

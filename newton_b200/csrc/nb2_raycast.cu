@@ -8,6 +8,9 @@
 //   intersect_ray_kernel   one thread per ray: the ray's own group, then the global group; per shape an AABB slab test, then the
 //                          reference's exact test (map_ray_to_local, ray_intersect_{plane, sphere, box, capsule, cylinder, cone,
 //                          ellipsoid}, ray_intersect_shape; ray_intersect_mesh for MESH / CONVEX_MESH shapes).
+//   camera_render_kernel   one thread per pixel of every (world, camera) image (reference SensorTiledCamera.update): the ray
+//                          generated from the camera's ray table and transform, then the same group walk as intersect_ray
+//                          (closest_hit_slots) with the camera's start distance, back-face culling and type rules.
 //
 // The reference walks a Warp BVH over the shapes, so its tie order is the traversal order.  Here the shapes of a group are
 // scanned in ascending shape id and a hit replaces the best one only when strictly closer: ties go to the earlier candidate.
@@ -331,8 +334,11 @@ __device__ Hit ray_cone(V3 o, V3 d, float radius, float hh) {
     return Hit{t_hit, unit(nl)};
 }
 
+// CULL (the camera's back-face culling, raycast.py:620-626): after the parallel test, a ray coming from behind (+z) misses.
+template <bool CULL>
 __device__ Hit ray_plane(V3 o, V3 d, V3 size) {
     if (fabsf(d.z) < RC_PARALLEL_TOL) return miss();
+    if (CULL && d.z > 0.0f) return miss();
     const float t = -o.z / d.z;
     if (t < 0.0f) return miss();
     const float hx = o.x + t * d.x, hy = o.y + t * d.y;
@@ -342,13 +348,15 @@ __device__ Hit ray_plane(V3 o, V3 d, V3 size) {
     return Hit{t, V3(0.0f, 0.0f, 1.0f)};
 }
 
-// ray_intersect_shape (raycast.py:795-870) for the primitive types
+// ray_intersect_shape (raycast.py:795-870) for the primitive types; any other type misses.  NORMAL = false leaves the world normal
+// zero (the depth-only camera), so the primitives' normal arithmetic is dead code there.
+template <bool CULL, bool NORMAL>
 __device__ Hit ray_shape(const Xf& X, V3 size, int type, V3 o, V3 d) {
     V3 ol, dl;
     map_ray_to_local(X, o, d, size, false, ol, dl);
     Hit h = miss();
     switch (type) {
-        case T_PLANE: h = ray_plane(ol, dl, size); break;
+        case T_PLANE: h = ray_plane<CULL>(ol, dl, size); break;
         case T_SPHERE: h = ray_sphere(ol, dl, size.x); break;
         case T_BOX: h = ray_box(ol, dl, size); break;
         case T_CAPSULE: h = ray_capsule(ol, dl, size.x, size.y); break;
@@ -357,7 +365,7 @@ __device__ Hit ray_shape(const Xf& X, V3 size, int type, V3 o, V3 d) {
         case T_ELLIPSOID: h = ray_ellipsoid(ol, dl, size); break;
         default: break;
     }
-    if (h.t >= 0.0f) return Hit{h.t, unit(xvec(X, h.n))};
+    if (h.t >= 0.0f) return Hit{h.t, NORMAL ? unit(xvec(X, h.n)) : V3()};
     return Hit{h.t, V3()};
 }
 
@@ -429,7 +437,10 @@ __device__ __forceinline__ bool slab(float o, float d, float lo, float hi, float
 }
 
 // ray_intersect_mesh (raycast.py:649-699) over the mesh's triangle BVH: closest (t, face) with 0 <= t < max_t, normal
-// normalize(safe_div(normalize(cross(b - a, c - a)), scale)) in the local frame.
+// normalize(safe_div(normalize(cross(b - a, c - a)), scale)) in the local frame.  CULL (raycast.py:684-691): when that closest
+// triangle faces away from the ray, dot(d, normalize(cross(b - a, c - a))) >= 0, the mesh yields no hit at all; it does not
+// fall back to a farther front-facing triangle.
+template <bool CULL>
 __device__ bool ray_mesh(const nb2_raycast_view& v, int mesh, V3 o, V3 d, float max_t, float& t_out, V3& n_out) {
     const int root = v.mesh_root[mesh];
     if (root < 0) return false;
@@ -484,6 +495,7 @@ __device__ bool ray_mesh(const nb2_raycast_view& v, int mesh, V3 o, V3 d, float 
     const V3 a = ld3(tv), b = ld3(tv + 3), c = ld3(tv + 6);
     t_out = best_t;
     n_out = unit(cross(b - a, c - a));
+    if (CULL && !(dot(d, n_out) < 0.0f)) return false;
     return true;
 }
 
@@ -596,6 +608,44 @@ __device__ __forceinline__ bool ray_aabb(V3 o, V3 d, V3 lo, V3 hi) {
     return t0 <= t1;
 }
 
+// The closest-hit walk over one group's slots [e0, e1), shared by intersect_ray_kernel and camera_render_kernel: per slot the AABB
+// pre-test, then the exact test of the slot's type.  `best` enters as the start distance (1e10 for intersect_ray, max_distance
+// for the camera) and a hit replaces the best one only when 0 <= t < best, so ties go to the earlier candidate.  A mesh is
+// queried with max_t = best.
+//   CULL    back-face culling of planes and meshes (the camera's RenderConfig.enable_backface_culling);
+//   HULLS   CONVEX_MESH shapes take the mesh path (intersect_ray).  Without it they fall through to ray_shape and never hit,
+//           as in the reference camera, whose closest hit sends only MESH to the mesh test (raytrace.py:126);
+//   NORMAL  compute the world normal (false: the depth-only camera).
+template <bool CULL, bool HULLS, bool NORMAL>
+__device__ __forceinline__ void closest_hit_slots(const nb2_raycast_view& v, int e0, int e1, V3 o, V3 d, float& best, int& best_id,
+                                                  V3& best_n) {
+    for (int e = e0; e < e1; ++e) {
+        if (!ray_aabb(o, d, ld3(v.table_lower + 3 * e), ld3(v.table_upper + 3 * e))) continue;
+        const Xf X = ldx(v.table_transform + 7 * e);
+        const V3 size = ld3(v.table_scale + 3 * e);
+        const int type = v.table_type[e];
+        Hit h;
+        if (type == T_MESH || (HULLS && type == T_CONVEX_MESH)) {
+            V3 ol, dl, nq;
+            map_ray_to_local(X, o, d, size, true, ol, dl);
+            float t;
+            const int mesh = v.table_mesh[e];
+            if (mesh >= 0 && ray_mesh<CULL>(v, mesh, ol, dl, best, t, nq)) {
+                h = Hit{t, NORMAL ? unit(xvec(X, unit(safe_div3(nq, size)))) : V3()};
+            } else {
+                h = miss();
+            }
+        } else {
+            h = ray_shape<CULL, NORMAL>(X, size, type, o, d);
+        }
+        if (h.t >= 0.0f && h.t < best) {
+            best = h.t;
+            best_id = v.enabled[e];
+            best_n = h.n;
+        }
+    }
+}
+
 __global__ void __launch_bounds__(128) intersect_ray_kernel(const nb2_raycast_view v, int ray_count, const float* __restrict__ origins,
                                                             const float* __restrict__ directions, const int* __restrict__ worlds,
                                                             int enable_global_world, float* out_dist, int* out_shape_id,
@@ -617,36 +667,67 @@ __global__ void __launch_bounds__(128) intersect_ray_kernel(const nb2_raycast_vi
             if (!enable_global_world || w < 0) continue;
             g = W;
         }
-        const int e1 = v.group_start[g + 1];
-        for (int e = v.group_start[g]; e < e1; ++e) {
-            if (!ray_aabb(o, d, ld3(v.table_lower + 3 * e), ld3(v.table_upper + 3 * e))) continue;
-            const Xf X = ldx(v.table_transform + 7 * e);
-            const V3 size = ld3(v.table_scale + 3 * e);
-            const int type = v.table_type[e];
-            Hit h;
-            if (type == T_MESH || type == T_CONVEX_MESH) {
-                V3 ol, dl, nq;
-                map_ray_to_local(X, o, d, size, true, ol, dl);
-                float t;
-                const int mesh = v.table_mesh[e];
-                if (mesh >= 0 && ray_mesh(v, mesh, ol, dl, best, t, nq)) {
-                    h = Hit{t, unit(xvec(X, unit(safe_div3(nq, size))))};
-                } else {
-                    h = miss();
-                }
-            } else {
-                h = ray_shape(X, size, type, o, d);
-            }
-            if (h.t >= 0.0f && h.t < best) {
-                best = h.t;
-                best_id = v.enabled[e];
-                best_n = h.n;
-            }
-        }
+        closest_hit_slots<false, true, true>(v, v.group_start[g], v.group_start[g + 1], o, d, best, best_id, best_n);
     }
     if (out_dist) out_dist[r] = best_id < 0 ? -1.0f : best;
     if (out_shape_id) out_shape_id[r] = best_id;
     if (out_normal) st3(out_normal + 3 * r, best_n);
+}
+
+// ---- tiled camera (reference SensorTiledCamera.update, sensors/warp_raytrace/render.py:86-345) --------------------------------
+// One thread per pixel.  A CTA of 4 warps renders a 16 x 8 pixel tile of one (world, camera) image and each warp an 8 x 4
+// sub-tile, so neighbouring rays share branches and mesh-BVH paths.  The grid is flat: blockIdx.x = (world * C + camera) *
+// tiles + tile, so worlds x cameras x tiles is bounded by gridDim.x (2^31 - 1), not gridDim.y.  Thread 0 does the per-image
+// work once (the camera transform, its forward axis and the two group ranges) and shares it through shared memory.
+constexpr int CAM_TILE_W = 16, CAM_TILE_H = 8, CAM_THREADS = 128;
+
+template <bool NORMAL, bool CULL>
+__global__ void __launch_bounds__(CAM_THREADS) camera_render_kernel(const nb2_raycast_view v, const nb2_camera_desc c, int tiles_x,
+                                                                    int tiles) {
+    __shared__ float s_xf[7], s_fwd[3];
+    __shared__ int s_range[4];
+    const int pair = blockIdx.x / tiles, tile = blockIdx.x - pair * tiles;
+    const int world = pair / c.camera_count, cam = pair - world * c.camera_count;
+    if (threadIdx.x == 0) {
+        const float* tp = c.camera_transforms + 7 * ((size_t)cam * c.world_count + world);
+        const Xf T = ldx(tp);
+        stx(s_xf, T);
+        st3(s_fwd, unit(xvec(T, V3(0.0f, 0.0f, -1.0f))));
+        const int W = v.world_count;
+        s_range[0] = v.group_start[world];
+        s_range[1] = v.group_start[world + 1];
+        const bool global = (c.flags & NB2_CAMERA_GLOBAL_WORLD) != 0;
+        s_range[2] = global ? v.group_start[W] : 0;
+        s_range[3] = global ? v.group_start[W + 1] : 0;
+    }
+    __syncthreads();
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int ty = tile / tiles_x, tx = tile - ty * tiles_x;
+    const int px = tx * CAM_TILE_W + (warp & 1) * 8 + (lane & 7);
+    const int py = ty * CAM_TILE_H + (warp >> 1) * 4 + (lane >> 3);
+    if (px >= c.width || py >= c.height) return;
+    const Xf T = ldx(s_xf);
+    const float* ray = c.camera_rays + 6 * (((size_t)cam * c.height + py) * c.width + px);
+    const V3 o = xpoint(T, ld3(ray)), d = xvec(T, ld3(ray + 3));
+    float best = c.max_distance;
+    int best_id = -1;
+    V3 best_n;
+    if (dot(d, d) > 1.0e-12f) {
+        closest_hit_slots<CULL, false, NORMAL>(v, s_range[0], s_range[1], o, d, best, best_id, best_n);
+        closest_hit_slots<CULL, false, NORMAL>(v, s_range[2], s_range[3], o, d, best, best_id, best_n);
+    }
+    const size_t out = ((size_t)pair * c.height + py) * c.width + px;
+    if (best_id < 0) {
+        if (c.depth) c.depth[out] = c.clear_depth;
+        if (c.forward_depth) c.forward_depth[out] = c.clear_depth;
+        if (c.shape_index) c.shape_index[out] = c.clear_shape_index;
+        if (NORMAL) st3(c.normal + 3 * out, V3(c.clear_normal[0], c.clear_normal[1], c.clear_normal[2]));
+        return;
+    }
+    if (c.depth) c.depth[out] = best;
+    if (c.forward_depth) c.forward_depth[out] = best * dot(d, ld3(s_fwd));
+    if (c.shape_index) c.shape_index[out] = (uint32_t)best_id;
+    if (NORMAL) st3(c.normal + 3 * out, best_n);
 }
 
 }  // namespace
@@ -664,6 +745,24 @@ nb2_status launch_intersect_ray(const nb2_raycast_view& v, int ray_count, const 
     if (ray_count == 0 || (!out_dist && !out_shape_id && !out_normal)) return NB2_OK;
     intersect_ray_kernel<<<(ray_count + 127) / 128, 128, 0, s>>>(v, ray_count, origins, directions, worlds, enable_global_world ? 1 : 0,
                                                                  out_dist, out_shape_id, out_normal);
+    count_launch(1);
+    NB2_CUDA_CHECK(cudaGetLastError());
+    return NB2_OK;
+}
+
+nb2_status launch_camera_render(const nb2_raycast_view& v, const nb2_camera_desc& c, cudaStream_t s) {
+    if (v.enabled_count == 0 || (!c.depth && !c.forward_depth && !c.shape_index && !c.normal)) return NB2_OK;
+    const int tiles_x = (c.width + CAM_TILE_W - 1) / CAM_TILE_W, tiles_y = (c.height + CAM_TILE_H - 1) / CAM_TILE_H;
+    const int tiles = tiles_x * tiles_y;
+    const unsigned blocks = (unsigned)c.world_count * (unsigned)c.camera_count * (unsigned)tiles;
+    const bool cull = (c.flags & NB2_CAMERA_BACKFACE_CULLING) != 0;
+    if (c.normal) {
+        if (cull) camera_render_kernel<true, true><<<blocks, CAM_THREADS, 0, s>>>(v, c, tiles_x, tiles);
+        else camera_render_kernel<true, false><<<blocks, CAM_THREADS, 0, s>>>(v, c, tiles_x, tiles);
+    } else {
+        if (cull) camera_render_kernel<false, true><<<blocks, CAM_THREADS, 0, s>>>(v, c, tiles_x, tiles);
+        else camera_render_kernel<false, false><<<blocks, CAM_THREADS, 0, s>>>(v, c, tiles_x, tiles);
+    }
     count_launch(1);
     NB2_CUDA_CHECK(cudaGetLastError());
     return NB2_OK;

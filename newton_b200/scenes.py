@@ -510,6 +510,50 @@ def range_ring_rays(model, body_q):
     return origins, directions, worlds
 
 
+CAMERA_SIZE = (64, 48)  # width, height of the quadrupeds' depth camera
+CAMERA_FOV_DEG = 58.0  # vertical field of view
+CAMERA_PITCH_DEG = 30.0  # pitched down from the base's heading
+CAMERA_MOUNT = (0.4, 0.0, 0.1)  # camera position in the base frame: at the front of the trunk, a little above its axis
+
+
+def _quat_mul_t(a, b):
+    ax, ay, az, aw = a.unbind(-1)
+    bx, by, bz, bw = b.unbind(-1)
+    return torch.stack([aw * bx + bw * ax + ay * bz - by * az, aw * by + bw * ay + az * bx - bz * ax,
+                        aw * bz + bw * az + ax * by - bx * ay, aw * bw - ax * bx - ay * by - az * bz], dim=-1)
+
+
+def camera_mount_quat(pitch_deg: float = CAMERA_PITCH_DEG) -> np.ndarray:
+    """Camera-to-base rotation of a camera looking along the base's +x with the base's +z up, pitched down by ``pitch_deg``.
+    The camera looks down its own -z with +y up (the pinhole rays of ``SensorTiledCamera.utils``)."""
+    level = X.quat_mul(X.quat_from_axis_angle((0.0, 0.0, 1.0), -0.5 * math.pi), X.quat_from_axis_angle((1.0, 0.0, 0.0), 0.5 * math.pi))
+    return np.asarray(X.quat_mul(level, X.quat_from_axis_angle((1.0, 0.0, 0.0), -math.radians(pitch_deg))), dtype=np.float64)
+
+
+_MOUNTS: dict = {}
+
+
+def quadruped_camera_transforms(model, body_q, mount=CAMERA_MOUNT, pitch_deg: float = CAMERA_PITCH_DEG):
+    """One camera per quadruped base, rigidly mounted on it: ``[1, world_count, 7]`` float32 camera-to-world transforms
+    (``SensorTiledCamera.update``'s ``(camera_count, world_count)`` order), base pose * mount."""
+    key = (id(model.body_world_start), str(body_q.device), tuple(mount), float(pitch_deg))
+    if key not in _MOUNTS:  # built once per device, so that later calls make no host copy and can be captured in a CUDA graph
+        _MOUNTS[key] = (torch.as_tensor(camera_mount_quat(pitch_deg), dtype=torch.float32, device=body_q.device),
+                        torch.as_tensor(mount, dtype=torch.float32, device=body_q.device),
+                        model.body_world_start[: model.world_count].long())
+    qm0, off0, base = _MOUNTS[key]
+    q_b = body_q[base, 3:7]
+    qm = qm0.expand_as(q_b)
+    off = off0.expand(q_b.shape[0], 3)
+    x, y, z, w = q_b.unbind(-1)
+    c = 2.0 * w * w - 1.0
+    d = 2.0 * (x * off[:, 0] + y * off[:, 1] + z * off[:, 2])
+    rot = torch.stack([off[:, 0] * c + x * d + (y * off[:, 2] - z * off[:, 1]) * w * 2.0,
+                       off[:, 1] * c + y * d + (z * off[:, 0] - x * off[:, 2]) * w * 2.0,
+                       off[:, 2] * c + z * d + (x * off[:, 1] - y * off[:, 0]) * w * 2.0], dim=-1)
+    return torch.cat([body_q[base, :3] + rot, _quat_mul_t(q_b, qm)], dim=-1)[None].contiguous()
+
+
 # Franka Emika Panda, from its published modified Denavit-Hartenberg table and joint ranges (a, d, alpha of frame i-1 -> i, metres /
 # radians) - 7 revolute joints, a fixed hand 0.107 m past the flange turned by -pi/4, two prismatic fingers 0.0584 m ahead of it.
 PANDA_DH = ((0.0, 0.333, 0.0), (0.0, 0.0, -0.5 * math.pi), (0.0, 0.316, 0.5 * math.pi), (0.0825, 0.0, 0.5 * math.pi),

@@ -1,4 +1,5 @@
 """Sensors (reference ``newton.sensors``)."""
 from .sensor_contact import SensorContact
+from .sensor_tiled_camera import ClearData, RenderConfig, RenderOrder, SensorTiledCamera, Utils
 
-__all__ = ["SensorContact"]
+__all__ = ["ClearData", "RenderConfig", "RenderOrder", "SensorContact", "SensorTiledCamera", "Utils"]
