@@ -196,6 +196,15 @@ typedef struct nb2_featherstone_params {
     int32_t use_tile_gemm;
 } nb2_featherstone_params;
 
+/* Constructor kwargs of reference SolverSemiImplicit (solvers/semi_implicit/solver_semi_implicit.py:72-121) that act on rigid bodies.
+   joint_attach_ke / joint_attach_kd are the stiffness and damping of the maximal-coordinate joint attachment springs. */
+typedef struct nb2_semi_implicit_params {
+    float angular_damping;
+    float friction_smoothing;
+    float joint_attach_ke;
+    float joint_attach_kd;
+} nb2_semi_implicit_params;
+
 typedef struct nb2_model nb2_model; /* opaque: env partition, contact blocks, solver scratch */
 
 /* --- lifecycle ------------------------------------------------------------------------------ */
@@ -287,6 +296,18 @@ nb2_status nb2_integrate_bodies(nb2_model* model, const nb2_state_view* state_in
 nb2_status nb2_featherstone_step(nb2_model* model, const nb2_featherstone_params* params,
                                  const nb2_state_view* state_in, const nb2_state_view* state_out,
                                  const nb2_control_view* control, int32_t use_contacts, float dt, void* cuda_stream);
+
+/* Reference SolverSemiImplicit.step (solvers/semi_implicit/solver_semi_implicit.py:124-217), rigid bodies: joint attachment springs
+ * and drives (eval_body_joints, kernels_body.py:54-520), penalty contacts (eval_body_contact, kernels_contact.py:381-556) and
+ * symplectic Euler (integrate_bodies, solvers/solver.py:112-170) in one launch.  `use_contacts` != 0 consumes the model's contact
+ * blocks (the last nb2_collide / nb2_contacts_import).  Writes state_out.body_q / body_qd only; state_in may be state_out.  When the
+ * model has no joints or control->joint_f is NULL (the reference's Control.joint_f = None), the accumulated forces are written back
+ * to state_in.body_f, as the reference accumulates into that array itself; otherwise state_in.body_f is left as it is.
+ * control->joint_f / joint_target_q / joint_target_qd must be non-NULL when the model has joint dofs; a model whose joints have no
+ * dofs may pass a NULL joint_f.  An environment too large for the kernel's shared memory is refused with NB2_ERR_UNSUPPORTED. */
+nb2_status nb2_semi_implicit_step(nb2_model* model, const nb2_semi_implicit_params* params, const nb2_state_view* state_in,
+                                  const nb2_state_view* state_out, const nb2_control_view* control, int32_t use_contacts, float dt,
+                                  void* cuda_stream);
 
 /* Reference newton.eval_fk (sim/articulation.py:500-574): joint_q/joint_qd -> body_q/body_qd. */
 nb2_status nb2_eval_fk(nb2_model* model, const float* joint_q, const float* joint_qd, float* body_q, float* body_qd,

@@ -281,6 +281,17 @@ class FeatherstoneParams(C.Structure):
     ]
 
 
+class SemiImplicitParams(C.Structure):
+    """``nb2_semi_implicit_params``"""
+
+    _fields_ = [
+        ("angular_damping", C.c_float),
+        ("friction_smoothing", C.c_float),
+        ("joint_attach_ke", C.c_float),
+        ("joint_attach_kd", C.c_float),
+    ]
+
+
 _COUNT_FIELDS = ("world_count", "body_count", "joint_count", "joint_dof_count", "joint_coord_count", "shape_count",
                  "articulation_count")
 

@@ -745,6 +745,18 @@ nb2_status nb2_featherstone_step(nb2_model* model, const nb2_featherstone_params
                                     static_cast<cudaStream_t>(cuda_stream));
 }
 
+nb2_status nb2_semi_implicit_step(nb2_model* model, const nb2_semi_implicit_params* params, const nb2_state_view* state_in,
+                                  const nb2_state_view* state_out, const nb2_control_view* control, int32_t use_contacts, float dt,
+                                  void* cuda_stream) {
+    if (!model || !params || !state_in || !state_out || !control) {
+        set_error("nb2_semi_implicit_step: NULL argument");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    DeviceGuard guard(model->device);
+    return launch_semi_implicit_step(model, *params, *state_in, *state_out, *control, use_contacts, dt,
+                                     static_cast<cudaStream_t>(cuda_stream));
+}
+
 nb2_status nb2_eval_fk(nb2_model* model, const float* joint_q, const float* joint_qd, float* body_q, float* body_qd,
                        void* cuda_stream) {
     if (!model || !joint_q || !joint_qd || !body_q || !body_qd) {

@@ -25,6 +25,7 @@
 
 #include "nb2_internal.cuh"
 #include "nb2_joint.cuh"
+#include "nb2_penalty.cuh"
 
 namespace nb2 {
 
@@ -434,61 +435,14 @@ featherstone_step_kernel(DevModel M, nb2_featherstone_params P, nb2_state_view s
     // side A before side B - the summation order of the reference's serial device, so the result is bit-identical.  The records
     // live in whichever dead block is larger: H (not formed yet) or v_s / a_s (dead between the RNEA forward pass and the closing FK).
     if (use_contacts) {
-        constexpr int CR = 11;  // odd stride: lanes = consecutive contacts hit different banks
+        constexpr int CR = kContactRecord;
         const int cap_h = M.max_env_H / CR, cap_v = (12 * M.max_env_bodies) / CR;
         float* crec = cap_h >= cap_v ? sm.H : sm.vs;
         const int ccap = cap_h >= cap_v ? cap_h : cap_v;  // >= 1: an environment has at least one body
         for (int cbase = 0; cbase < nc; cbase += ccap) {
             const int cend = min(nc, cbase + ccap);
-            for (int c = cbase + l; c < cend; c += L) {
-                const int s = slot0 + c;
-                const int ba = __float_as_int(cb[CF_BODY_A * T + s]), bb = __float_as_int(cb[CF_BODY_B * T + s]);
-                float* rec = crec + (c - cbase) * CR;
-                int code = 0;
-                if (ba >= 0 || bb >= 0) {
-                    const float ke = cb[CF_KE * T + s], kd = cb[CF_KD * T + s], kf = cb[CF_KF * T + s], ka = cb[CF_KA * T + s], mu = cb[CF_MU * T + s];
-                    const V3 n = -V3(cb[CF_NX * T + s], cb[CF_NY * T + s], cb[CF_NZ * T + s]);
-                    V3 bx_a(cb[CF_P0X * T + s], cb[CF_P0Y * T + s], cb[CF_P0Z * T + s]);
-                    V3 bx_b(cb[CF_P1X * T + s], cb[CF_P1Y * T + s], cb[CF_P1Z * T + s]);
-                    V3 r_a, r_b;
-                    if (ba >= 0) {
-                        const Xf X = ldx(sm.bq + 7 * ba);
-                        bx_a = xpoint(X, bx_a) - cb[CF_MARGIN0 * T + s] * n;
-                        r_a = bx_a - xpoint(X, ld3(d.body_com + 3 * (b0 + ba)));
-                    }
-                    if (bb >= 0) {
-                        const Xf X = ldx(sm.bq + 7 * bb);
-                        bx_b = xpoint(X, bx_b) + cb[CF_MARGIN1 * T + s] * n;
-                        r_b = bx_b - xpoint(X, ld3(d.body_com + 3 * (b0 + bb)));
-                    }
-                    const float dd = dot(n, bx_a - bx_b);
-                    if (dd < ka) {
-                        V3 bv_a, bv_b;
-                        if (ba >= 0) bv_a = ld3(sm.qdfk + 6 * ba) + cross(ld3(sm.qdfk + 6 * ba + 3), r_a);
-                        if (bb >= 0) bv_b = ld3(sm.qdfk + 6 * bb) + cross(ld3(sm.qdfk + 6 * bb + 3), r_b);
-                        const V3 v = bv_a - bv_b;
-                        const float vn = dot(n, v);
-                        const V3 vt = v - n * vn;
-                        const float fn = dd * ke;
-                        const float fd = fmin_w(vn, 0.0f) * kd * (dd < 0.0f ? 1.0f : 0.0f);
-                        V3 ft;
-                        if (dd < 0.0f) {
-                            const float a2 = dot(vt, vt), delta = P.friction_smoothing;
-                            const float vs = (a2 <= delta * delta) ? 0.5f * a2 : delta * (sqrtf(a2) - 0.5f * delta);
-                            if (vs > 0.0f) {
-                                const V3 fr = vt / vs;
-                                ft = fr * fmin_w(kf * vs, -mu * (fn + fd));
-                            }
-                        }
-                        const V3 f_total = n * (fn + fd) + ft;
-                        st3(rec, f_total);
-                        st3(rec + 3, cross(r_a, f_total));
-                        st3(rec + 6, cross(r_b, f_total));
-                        code = (ba + 1) | ((bb + 1) << 16);
-                    }
-                }
-                reinterpret_cast<int*>(rec)[9] = code;  // 0 = no contribution (beyond the adhesion distance / no body)
-            }
+            for (int c = cbase + l; c < cend; c += L)
+                penalty_contact_record(cb, T, slot0 + c, d, b0, sm.bq, sm.qdfk, P.friction_smoothing, crec + (c - cbase) * CR);
             __syncwarp(gmask);
             for (int b = l; b < nb; b += L) {
                 V3 facc = ld3(sm.fe + 6 * b), tacc = ld3(sm.fe + 6 * b + 3);
@@ -1120,29 +1074,6 @@ nb2_status launch_eval_fk(nb2_model* m, const float* joint_q, const float* joint
 }
 
 // ---- public newton.eval_ik (sim/articulation.py:640-932 eval_articulation_ik): one thread per joint -----------------------------
-NB2_DEV float twist_angle_signed(V3 axis, Q4 q) {  // wp.quat_twist_angle_signed: 2 atan2(q.xyz . axis, q.w), range (-2 pi, 2 pi]
-    return 2.0f * atan2_w(dot(V3(q.x, q.y, q.z), axis), q.w);
-}
-
-// newton.math.quat_decompose (math/spatial.py:150-175): wp.quat_to_euler(q, 2, 1, 0), each angle wrapped to [-pi, pi); for
-// q = qx(a) qy(b) qz(c) the result is (a, b, c)
-NB2_DEV float wrap_pm_pi(float theta) {
-    const float pi = 3.14159265358979323846f, two_pi = 2.0f * pi;
-    float wrapped = fmodf(theta + pi, two_pi);
-    if (wrapped < 0.0f) wrapped += two_pi;
-    return wrapped - pi;
-}
-NB2_DEV V3 q_decompose(Q4 q) {
-    const float a = q.w - q.y, b = q.z - q.x, c = q.y + q.w, d = -q.x - q.z;
-    const float n_ab = a * a + b * b;
-    float theta2 = acos_w(2.0f * n_ab / (n_ab + c * c + d * d) - 1.0f);
-    const float theta_plus = atan2_w(b, a), theta_minus = atan2_w(d, c);
-    const float theta1 = theta_plus - theta_minus;
-    float theta3 = theta_plus + theta_minus;
-    theta3 = -theta3;
-    theta2 -= 1.57079632679489661923f;
-    return V3(wrap_pm_pi(theta3), wrap_pm_pi(theta2), wrap_pm_pi(theta1));
-}
 // invert_2d / invert_3d_rotational_dofs (sim/articulation.py:85-126, 177-236); `three` selects the 3-axis variant
 NB2_DEV void invert_rotational_dofs(bool three, V3 axis_0, V3 axis_1, V3 axis_2, Q4 q_p, Q4 q_c, V3 w_err, float* angles_out, float* vel_out) {
     const V3 axis_2_rh = cross(axis_0, axis_1);

@@ -235,6 +235,9 @@ nb2_status launch_integrate_bodies(nb2_model* m, const nb2_state_view& in, const
 nb2_status launch_featherstone_step(nb2_model* m, const nb2_featherstone_params& p, const nb2_state_view& in,
                                     const nb2_state_view& out, const nb2_control_view& ctl, int use_contacts, float dt,
                                     cudaStream_t s);
+nb2_status launch_semi_implicit_step(nb2_model* m, const nb2_semi_implicit_params& p, const nb2_state_view& in,
+                                     const nb2_state_view& out, const nb2_control_view& ctl, int use_contacts, float dt,
+                                     cudaStream_t s);
 nb2_status launch_eval_fk(nb2_model* m, const float* joint_q, const float* joint_qd, float* body_q, float* body_qd,
                           cudaStream_t s, const uint8_t* mask = nullptr, const int* indices = nullptr, int index_count = 0,
                           int body_flag_filter = 3);

@@ -199,4 +199,28 @@ NB2_DEV void axes3(V3 a0, V3 a1, V3 a2, float q0, float q1, V3& o0, V3& o1, V3& 
     o0 = a0; o1 = a1w; o2 = a2w;
 }
 
+NB2_DEV float twist_angle_signed(V3 axis, Q4 q) {  // wp.quat_twist_angle_signed: 2 atan2(q.xyz . axis, q.w), range (-2 pi, 2 pi]
+    return 2.0f * atan2_w(dot(V3(q.x, q.y, q.z), axis), q.w);
+}
+
+// newton.math.quat_decompose (math/spatial.py:150-175): wp.quat_to_euler(q, 2, 1, 0), each angle wrapped to [-pi, pi); for
+// q = qx(a) qy(b) qz(c) the result is (a, b, c)
+NB2_DEV float wrap_pm_pi(float theta) {
+    const float pi = 3.14159265358979323846f, two_pi = 2.0f * pi;
+    float wrapped = fmodf(theta + pi, two_pi);
+    if (wrapped < 0.0f) wrapped += two_pi;
+    return wrapped - pi;
+}
+NB2_DEV V3 q_decompose(Q4 q) {
+    const float a = q.w - q.y, b = q.z - q.x, c = q.y + q.w, d = -q.x - q.z;
+    const float n_ab = a * a + b * b;
+    float theta2 = acos_w(2.0f * n_ab / (n_ab + c * c + d * d) - 1.0f);
+    const float theta_plus = atan2_w(b, a), theta_minus = atan2_w(d, c);
+    const float theta1 = theta_plus - theta_minus;
+    float theta3 = theta_plus + theta_minus;
+    theta3 = -theta3;
+    theta2 -= 1.57079632679489661923f;
+    return V3(wrap_pm_pi(theta3), wrap_pm_pi(theta2), wrap_pm_pi(theta1));
+}
+
 }  // namespace nb2
