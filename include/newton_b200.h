@@ -264,9 +264,13 @@ nb2_status nb2_contacts_sort(nb2_model* model, const nb2_contacts_view* contacts
 
 /* Load a reference-layout `Contacts` buffer that nb2_collide did NOT produce (e.g. written by the reference's own
  * CollisionPipeline, sim/collide.py:1765-2207, or by user code) into the model's env-major contact blocks, so that the next
- * nb2_xpbd_step / nb2_featherstone_step consumes it.  Contacts keep their array order inside each environment (stable sort
- * by world), i.e. the per-body summation order of the reference's serial device; contacts between two static shapes are
- * skipped; an environment's contacts beyond its block capacity (5 per candidate pair) are dropped.  The first call (and any
+ * nb2_xpbd_step / nb2_featherstone_step / nb2_semi_implicit_step consumes it.  Contacts keep their array order inside each
+ * environment (stable sort by world), i.e. the per-body summation order of the reference's serial device.  A negative shape id
+ * is a missing side, as upstream: the contact is against a fixed world point (its point is in world coordinates), that side
+ * has no body, and the materials are those of the one shape present.  Skipped, because they move nothing or have no
+ * environment: contacts whose two shape ids are equal, contacts that involve no body (two static shapes, or a static shape and
+ * a world point) and, in a model of several worlds, contacts whose shapes are all global (world -1).  An environment's contacts
+ * beyond its block capacity (5 per candidate pair) are dropped.  The first call (and any
  * call with a larger rigid_contact_max) allocates scratch and is therefore not CUDA-graph capturable; later calls are. */
 nb2_status nb2_contacts_import(nb2_model* model, const nb2_contacts_view* contacts, void* cuda_stream);
 

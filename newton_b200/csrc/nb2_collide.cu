@@ -1365,12 +1365,15 @@ __global__ void __launch_bounds__(256) import_keys_kernel(DevModel M, nb2_contac
     const int n = min(in.rigid_contact_count[0], in.rigid_contact_max);
     int key = M.env_count;  // sentinel: sorts behind every environment
     if (i < n) {
+        // a negative shape id is a missing side: the contact is against a fixed world point (kernels_contact.py:427-444)
         const int s0 = in.shape0[i], s1 = in.shape1[i];
-        if (s0 >= 0 && s1 >= 0 && s0 != s1 && s0 < d.shape_count && s1 < d.shape_count) {
-            const bool dynamic = d.shape_body[s0] >= 0 || d.shape_body[s1] >= 0;  // static-vs-static contacts move nothing
+        const bool h0 = s0 >= 0, h1 = s1 >= 0;
+        if ((h0 || h1) && s0 != s1 && s0 < d.shape_count && s1 < d.shape_count) {
+            // contacts that involve no body (static-vs-static, static-vs-point) move nothing
+            const bool dynamic = (h0 && d.shape_body[s0] >= 0) || (h1 && d.shape_body[s1] >= 0);
             int env = 0;
-            if (!implicit_single) {
-                const int w0 = d.shape_world[s0], w1 = d.shape_world[s1];
+            if (!implicit_single) {  // the world of a shape present; a contact whose shapes are all global has no environment
+                const int w0 = h0 ? d.shape_world[s0] : -1, w1 = h1 ? d.shape_world[s1] : -1;
                 env = w0 >= 0 ? w0 : w1;
             }
             if (dynamic && env >= 0 && env < M.env_count) key = env;
@@ -1378,6 +1381,15 @@ __global__ void __launch_bounds__(256) import_keys_kernel(DevModel M, nb2_contac
     }
     keys[i] = key;
     idx[i] = i;
+}
+
+// the reference's material average over the shapes present: the sum divided by their count as a float (kernels_contact.py:445-450)
+NB2_DEV float shape_material_mean(const float* mat, int sa, int sb) {
+    float sum = 0.0f;
+    int count = 0;
+    if (sa >= 0) sum += mat[sa], ++count;
+    if (sb >= 0) sum += mat[sb], ++count;
+    return sum / float(count);
 }
 
 NB2_DEV int lower_bound_int(const int* a, int n, int v) {
@@ -1406,8 +1418,8 @@ __global__ void __launch_bounds__(128) import_scatter_kernel(DevModel M, nb2_con
     const size_t T = size_t(M.slot_total);
     for (int c = lane; c < n; c += 32) {
         const int i = idx_sorted[first + c], slot = slot0 + c;
-        const int sa = in.shape0[i], sb = in.shape1[i];
-        const int body0 = d.shape_body[sa], body1 = d.shape_body[sb];
+        const int sa = max(in.shape0[i], -1), sb = max(in.shape1[i], -1);  // -1: no shape on that side (one-sided contact)
+        const int body0 = sa >= 0 ? d.shape_body[sa] : -1, body1 = sb >= 0 ? d.shape_body[sb] : -1;
         cb[CF_BODY_A * T + slot] = __int_as_float(body0 >= 0 ? body0 - bs : -1);
         cb[CF_BODY_B * T + slot] = __int_as_float(body1 >= 0 ? body1 - bs : -1);
         cb[CF_SHAPE0 * T + slot] = __int_as_float(sa);
@@ -1422,14 +1434,14 @@ __global__ void __launch_bounds__(128) import_scatter_kernel(DevModel M, nb2_con
         }
         cb[CF_MARGIN0 * T + slot] = in.margin0[i];
         cb[CF_MARGIN1 * T + slot] = in.margin1[i];
-        // pair-averaged coefficients, exactly as the collide kernel's write-out computes them
-        cb[CF_MU * T + slot] = (d.shape_material_mu[sa] + d.shape_material_mu[sb]) / 2.0f;
-        cb[CF_MU_TORSIONAL * T + slot] = (d.shape_material_mu_torsional[sa] + d.shape_material_mu_torsional[sb]) / 2.0f;
-        cb[CF_MU_ROLLING * T + slot] = (d.shape_material_mu_rolling[sa] + d.shape_material_mu_rolling[sb]) / 2.0f;
-        cb[CF_KE * T + slot] = 0.5f * (d.shape_material_ke[sa] + d.shape_material_ke[sb]);
-        cb[CF_KD * T + slot] = 0.5f * (d.shape_material_kd[sa] + d.shape_material_kd[sb]);
-        cb[CF_KF * T + slot] = 0.5f * (d.shape_material_kf[sa] + d.shape_material_kf[sb]);
-        cb[CF_KA * T + slot] = 0.5f * (d.shape_material_ka[sa] + d.shape_material_ka[sb]);
+        // coefficients averaged over the shapes present; for a pair, (a + b) / 2 has the bits of the collide kernel's write-out
+        cb[CF_MU * T + slot] = shape_material_mean(d.shape_material_mu, sa, sb);
+        cb[CF_MU_TORSIONAL * T + slot] = shape_material_mean(d.shape_material_mu_torsional, sa, sb);
+        cb[CF_MU_ROLLING * T + slot] = shape_material_mean(d.shape_material_mu_rolling, sa, sb);
+        cb[CF_KE * T + slot] = shape_material_mean(d.shape_material_ke, sa, sb);
+        cb[CF_KD * T + slot] = shape_material_mean(d.shape_material_kd, sa, sb);
+        cb[CF_KF * T + slot] = shape_material_mean(d.shape_material_kf, sa, sb);
+        cb[CF_KA * T + slot] = shape_material_mean(d.shape_material_ka, sa, sb);
     }
 }
 

@@ -1064,10 +1064,11 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
                 float active = 0.0f;
                 if (ba != bb) {
                     const int sa = __float_as_int(cb[CF_SHAPE0 * T + s]), sb = __float_as_int(cb[CF_SHAPE1 * T + s]);
-                    float restitution = 0.0f;
-                    restitution += d.shape_material_restitution[sa];
-                    restitution += d.shape_material_restitution[sb];
-                    restitution /= 2.0f;
+                    float restitution = 0.0f;  // averaged over the shapes present: an imported contact may have one (sa or sb = -1)
+                    int mat_nonzero = 0;
+                    if (sa >= 0) restitution += d.shape_material_restitution[sa], ++mat_nonzero;
+                    if (sb >= 0) restitution += d.shape_material_restitution[sb], ++mat_nonzero;
+                    restitution /= float(mat_nonzero);
                     const float* ra_rec = ba >= 0 ? bodies + ba * BR_SIZE : nullptr;
                     const float* rb_rec = bb >= 0 ? bodies + bb * BR_SIZE : nullptr;
                     const Xf Xa = ba >= 0 ? ldx(init_qd + ba * 13) : Xf(), Xb = bb >= 0 ? ldx(init_qd + bb * 13) : Xf();

@@ -131,3 +131,71 @@ def fixed_root_and_link_model(world_count: int = 2):
         b.end_world()
     b.add_ground_plane()
     return b.finalize()
+
+
+def one_sided_model(world_count: int = 3, boxes: int = 3):
+    """Per world, ``boxes`` free boxes just touching the ground (bottom face 1 mm below z = 0) and one static box resting on it,
+    with materials that differ from the ground's, so that averaging over one shape and over two give different coefficients."""
+    from newton_b200.sim.builder import ShapeConfig
+
+    b = ModelBuilder()
+    box_cfg = ShapeConfig(ke=3.0e3, kd=60.0, kf=700.0, ka=0.002, mu=0.7, restitution=0.3, mu_torsional=0.01, mu_rolling=0.001)
+    static_cfg = ShapeConfig(ke=5.0e3, kd=20.0, kf=300.0, ka=0.001, mu=0.4, restitution=0.1)
+    for w in range(world_count):
+        b.begin_world()
+        for i in range(boxes):
+            yaw = X.quat_from_axis_angle((0.0, 0.0, 1.0), 0.2 * i - 0.1 * w)
+            body = b.add_body(xform=X.transform((0.5 * i, 0.3 * w, 0.099), yaw), mass=1.0 + 0.2 * i)
+            b.add_shape_box(body, hx=0.1, hy=0.1, hz=0.1, cfg=box_cfg)
+        b.add_shape_box(-1, xform=X.transform((-0.5, 0.3 * w, 0.1)), hx=0.1, hy=0.1, hz=0.1, cfg=static_cfg)
+        b.end_world()
+    b.add_ground_plane()
+    model = b.finalize()
+    g = torch.Generator().manual_seed(world_count)
+    model.body_qd.copy_(torch.rand(model.body_qd.shape, generator=g) * 0.4 - 0.2)
+    return model
+
+
+def one_sided_contacts(model, device):
+    """A hand-written Contacts buffer over ``one_sided_model``: per box, a contact with the ground, one against a fixed world point
+    with shape1 = -1, one with shape0 = -1, and one whose two shape ids are equal; per world, a static-static pair (static box on
+    the ground) and a one-sided contact of the static box.  Worlds are interleaved and the margins are not zero.  Points of the
+    -1 side and of static shapes are world points."""
+    from newton_b200.sim.model import Contacts
+
+    shape_body = model.shape_body.cpu().numpy()
+    shape_world = model.shape_world.cpu().numpy()
+    body_q = model.body_q.cpu().numpy()
+    plane = int(np.nonzero((shape_body < 0) & (shape_world < 0))[0][0])
+    statics = [int(s) for s in np.nonzero((shape_body < 0) & (shape_world >= 0))[0]]
+    boxes = [int(s) for s in np.nonzero(shape_body >= 0)[0]]
+    rows = []  # (shape0, shape1, point0, point1, normal, margin0, margin1)
+    for k, s in enumerate(boxes):
+        x = body_q[shape_body[s], :3]
+        cx, cy = (0.1, -0.1)[k % 2], (0.1, -0.1)[(k // 2) % 2]
+        rows.append((s, plane, (cx, cy, -0.1), (x[0] + cx, x[1] + cy, 0.0), (0.0, 0.0, -1.0), 0.0, 0.0))
+        rows.append((s, -1, (-cx, cy, -0.1), (x[0] - cx, x[1] + cy, 0.0005), (0.0, 0.0, -1.0), 0.0005, 0.0))
+        rows.append((-1, s, (x[0] + cx, x[1] - cy, -0.0005), (cx, -cy, -0.1), (0.0, 0.0, 1.0), 0.0, 0.001))
+        rows.append((s, s, (0.0, 0.0, -0.1), (0.0, 0.0, -0.1), (0.0, 0.0, -1.0), 0.0, 0.0))
+    for s in statics:
+        rows.append((s, plane, (0.0, 0.0, -0.001), (0.0, 0.0, 0.0), (0.0, 0.0, -1.0), 0.0, 0.0))
+        rows.append((-1, s, (0.0, 0.0, 0.0), (0.0, 0.0, -0.001), (0.0, 0.0, 1.0), 0.0, 0.0))
+    # interleave the worlds: sort by (position inside the world's run, world) so that consecutive rows belong to different worlds
+    world_of = [int(shape_world[r[0] if r[0] >= 0 else r[1]]) for r in rows]
+    pos, seen = [], {}
+    for w in world_of:
+        pos.append(seen.get(w, 0))
+        seen[w] = pos[-1] + 1
+    order = sorted(range(len(rows)), key=lambda i: (pos[i], world_of[i]))
+    rows = [rows[i] for i in order]
+    c = Contacts(len(rows) + 5, 0, device=device, requested_attributes=model._requested_contact_attributes)
+    c.rigid_contact_count.fill_(len(rows))
+    for k, (s0, s1, p0, p1, nrm, m0, m1) in enumerate(rows):
+        c.rigid_contact_shape0[k] = s0
+        c.rigid_contact_shape1[k] = s1
+        c.rigid_contact_point0[k] = torch.tensor(p0)
+        c.rigid_contact_point1[k] = torch.tensor(p1)
+        c.rigid_contact_normal[k] = torch.tensor(nrm)
+        c.rigid_contact_margin0[k] = m0
+        c.rigid_contact_margin1[k] = m1
+    return c

@@ -363,3 +363,184 @@ def test_global_gravity_bodies(si):
     qd = s_out.body_qd.numpy()
     assert qd[global_body, 2] == pytest.approx(-0.2, abs=1e-6)
     assert qd[local_body, 2] == pytest.approx(-0.5, abs=1e-6)
+
+
+# ---- test_body_velocity.py:124-372 with the semi_implicit row of :871 (body_qd set directly, tolerance 1e-4) -------------------
+# test_semi_implicit.py's test_applied_body_force_and_kinematic_body drives a body whose COM is at its origin; none of these rows
+# (a COM away from the body origin, body_qd given at the COM) was covered.
+COM_OFFSETS = [(0.5, 0.0, 0.0), (0.0, 0.3, 0.0), (0.0, 0.0, 0.4), (0.2, 0.3, 0.1)]
+AXIS_VECTORS = [(0.0, 0.0, 1.0), (0.0, 1.0, 0.0), (1.0, 0.0, 0.0)]
+LINEAR_VELOCITIES = [(0.7, 0.0, 0.0), (0.0, 0.7, 0.0), (0.0, 0.0, 0.7)]
+
+
+def _offset_com_box(com, pos, rot=None):
+    """One free box (add_body) at ``pos`` whose COM is moved to ``com`` after its shape is added, without gravity."""
+    import oracle
+
+    b = ModelBuilder(gravity=(0.0, 0.0, 0.0))
+    body = b.add_body(xform=X.transform(pos, rot) if rot is not None else X.transform(pos))
+    b.add_shape_box(body, hx=0.1, hy=0.1, hz=0.1)
+    b.body_com[body] = np.asarray(com, dtype=np.float64)
+    model = b.finalize()
+    s0, s1 = model.state(), model.state()
+    oracle.eval_fk(model, model.joint_q, model.joint_qd, s0)
+    return model, s0, s1
+
+
+def _com_world(model, state):
+    q = state.body_q.numpy()[0].astype(np.float64)
+    from scipy.spatial.transform import Rotation
+
+    return q[:3] + Rotation.from_quat(q[3:]).apply(model.body_com.numpy()[0].astype(np.float64))
+
+
+def _free_steps(si, model, s0, s1, n, dt, control=None, wrench=None):
+    solver = _solver(si, model)
+    for _ in range(n):
+        solver.step(s0, s1, control, None, dt)
+        s0, s1 = s1, s0
+        if wrench is not None:  # re-applied for the next step, as the reference does
+            s0.body_f.copy_(wrench)
+            s1.body_f.copy_(wrench)
+    return s0
+
+
+@pytest.mark.parametrize("com", COM_OFFSETS)
+@pytest.mark.parametrize("w", AXIS_VECTORS)
+def test_body_velocity_angular_com_stationary(si, com, w):
+    """:124-211 - angular velocity alone turns the body about its COM: the COM moves < 1e-4 in 10 steps of 10 ms."""
+    model, s0, s1 = _offset_com_box(com, (1.0, 2.0, 3.0))
+    s0.body_qd.copy_(torch.tensor([[0.0, 0.0, 0.0, *w]]))
+    q0, c0 = s0.body_q.numpy()[0].copy(), _com_world(model, s0)
+    s = _free_steps(si, model, s0, s1, 10, 0.01)
+    assert np.linalg.norm(_com_world(model, s) - c0) < 1e-4
+    assert abs(float(np.dot(q0[3:], s.body_q.numpy()[0, 3:]))) < 0.9999
+
+
+@pytest.mark.parametrize("com", COM_OFFSETS)
+@pytest.mark.parametrize("v", LINEAR_VELOCITIES)
+def test_body_velocity_linear_com_moves(si, com, v):
+    """:214-287 - linear velocity alone moves the COM by v t, within 1e-4."""
+    model, s0, s1 = _offset_com_box(com, (0.0, 0.0, 1.0))
+    s0.body_qd.copy_(torch.tensor([[*v, 0.0, 0.0, 0.0]]))
+    c0 = _com_world(model, s0)
+    s = _free_steps(si, model, s0, s1, 10, 0.01)
+    assert np.linalg.norm(_com_world(model, s) - c0 - np.array(v) * 0.1) < 1e-4
+
+
+@pytest.mark.parametrize("com", COM_OFFSETS)
+def test_body_velocity_combined(si, com):
+    """:290-371 - (0.1, 0, 0) m/s and (0, 0, 1) rad/s together: the COM moves by v t within 1e-4 and the body turns."""
+    model, s0, s1 = _offset_com_box(com, (0.0, 0.0, 1.0))
+    s0.body_qd.copy_(torch.tensor([[0.1, 0.0, 0.0, 0.0, 0.0, 1.0]]))
+    q0, c0 = s0.body_q.numpy()[0].copy(), _com_world(model, s0)
+    s = _free_steps(si, model, s0, s1, 10, 0.01)
+    assert np.linalg.norm(_com_world(model, s) - c0 - np.array([0.01, 0.0, 0.0])) < 1e-4
+    assert abs(float(np.dot(q0[3:], s.body_q.numpy()[0, 3:]))) < 0.9999
+
+
+# ---- test_body_force.py:356-528 with the semi_implicit row of :551 (non-zero COM) ------------------------------------------------
+def _rotated_offset_com_box(com):
+    return _offset_com_box(com, (0.0, 0.0, 1.0), X.quat_from_axis_angle((1.0, 0.0, 0.0), 0.5 * np.pi))
+
+
+def _apply(model, s0, s1, wrench, use_control):
+    w = torch.tensor([wrench], dtype=torch.float32)
+    if use_control:
+        control = model.control()
+        control.joint_f.copy_(w[0])
+        return control, None
+    s0.body_f.copy_(w)
+    s1.body_f.copy_(w)
+    return None, w
+
+
+@pytest.mark.parametrize("use_control", [False, True])
+@pytest.mark.parametrize("com", COM_OFFSETS)
+@pytest.mark.parametrize("direction", LINEAR_VELOCITIES)
+def test_body_force_no_rotation(si, com, direction, use_control):
+    """:356-444 - a 10 N force at the COM of a rotated box (body_f or Control.joint_f), 5 steps of 10 ms: no angular velocity
+    (< 1e-3) and F / m t along the force within 5 %."""
+    model, s0, s1 = _rotated_offset_com_box(com)
+    f = np.array(direction) / 0.7 * 10.0
+    control, wrench = _apply(model, s0, s1, [*f, 0.0, 0.0, 0.0], use_control)
+    s = _free_steps(si, model, s0, s1, 5, 0.01, control, wrench)
+    qd = s.body_qd.numpy()[0]
+    expected = 10.0 / float(model.body_mass[0]) * 0.05
+    assert np.abs(qd[3:]).max() < 1e-3
+    assert float(np.dot(f / 10.0, qd[:3])) == pytest.approx(expected, abs=5e-2 * expected)
+
+
+@pytest.mark.parametrize("use_control", [False, True])
+@pytest.mark.parametrize("com", COM_OFFSETS)
+def test_body_force_combined_force_torque(si, com, use_control):
+    """:447-528 - 10 N along x and 10 Nm about z, 10 steps of 10 ms: v_x = F / m t and w_z = tau / I_zz t within 5 % of (1 + x),
+    every other component < 1e-3."""
+    model, s0, s1 = _rotated_offset_com_box(com)
+    control, wrench = _apply(model, s0, s1, [10.0, 0.0, 0.0, 0.0, 0.0, 10.0], use_control)
+    s = _free_steps(si, model, s0, s1, 10, 0.01, control, wrench)
+    qd = s.body_qd.numpy()[0]
+    v = 10.0 / float(model.body_mass[0]) * 0.1
+    w = 10.0 / float(model.body_inertia[0, 2, 2]) * 0.1
+    assert qd[0] == pytest.approx(v, abs=5e-2 * (1 + v))
+    assert qd[5] == pytest.approx(w, abs=5e-2 * (1 + w))
+    assert np.abs(qd[[1, 2, 3, 4]]).max() < 1e-3
+
+
+# ---- test_rigid_contact.py:28-235 (test_shapes_on_plane), semi_implicit row --------------------------------------------------------
+def test_shapes_on_plane(si):
+    """Spheres, lying capsules, boxes, upright cylinders and a triangle-mesh cube whose vertices are offset by (1, 0, 0) from its
+    origin, at two sizes, dropped from 0.5 m: ke 1e4, kd 1e3, kf 0, gap 0.1; SolverSemiImplicit(angular_damping=0.15,
+    friction_smoothing=2.0); 120 frames of 30 substeps at 60 fps.  At the end |v| and |w| < 0.2, positions within 0.25 of the
+    resting heights and quaternions within 0.1 of identity.  The mesh goes through CollisionPipeline(reduce_contacts=False), its
+    route here (one contact per vertex near the plane)."""
+    import oracle
+    from newton_b200.geometry.mesh import Mesh
+
+    s = 0.3
+    corners = [(-s, -s, -s), (-s, -s, s), (-s, s, s), (-s, s, -s), (s, -s, -s), (s, -s, s), (s, s, s), (s, s, -s),
+               (-s, -s, -s), (-s, -s, s), (s, -s, s), (s, -s, -s), (-s, s, -s), (-s, s, s), (s, s, s), (s, s, -s),
+               (-s, -s, -s), (-s, s, -s), (s, s, -s), (s, -s, -s), (-s, -s, s), (-s, s, s), (s, s, s), (s, -s, s)]
+    vertices = np.array(corners, dtype=np.float32) + np.array([1.0, 0.0, 0.0], dtype=np.float32)
+    indices = [0, 1, 2, 0, 2, 3, 4, 6, 5, 4, 7, 6, 8, 10, 9, 8, 11, 10, 12, 13, 14, 12, 14, 15, 16, 17, 18, 16, 18, 19,
+               20, 22, 21, 20, 23, 22]
+    cube = Mesh(vertices, np.array(indices, dtype=np.int32))
+    b = ModelBuilder()
+    cfg = b.default_shape_cfg
+    cfg.ke, cfg.kd, cfg.kf, cfg.gap = 1e4, 1000.0, 0.0, 0.1
+    expected = []
+    z_to_y = X.quat_between_vectors((0.0, 0.0, 1.0), (0.0, 1.0, 0.0))
+    for i, scale in enumerate((0.5, 1.0)):
+        y = 1.5 * i
+        body = b.add_body(xform=X.transform((0.0, y, 0.5)))
+        b.add_shape_sphere(body, radius=0.1 * scale)
+        expected.append((0.0, y, 0.1 * scale))
+        body = b.add_body(xform=X.transform((2.0, y, 0.5)))
+        b.add_shape_capsule(body, xform=X.transform((0.0, 0.0, 0.0), z_to_y), radius=0.1 * scale, half_height=0.3 * scale)
+        expected.append((2.0, y, 0.1 * scale))
+        body = b.add_body(xform=X.transform((4.0, y, 0.5)))
+        b.add_shape_box(body, hx=0.2 * scale, hy=0.25 * scale, hz=0.3 * scale)
+        expected.append((4.0, y, 0.3 * scale))
+        body = b.add_body(xform=X.transform((5.0, y, 0.5)))
+        b.add_shape_cylinder(body, radius=0.1 * scale, half_height=0.3 * scale)
+        expected.append((5.0, y, 0.3 * scale))
+        body = b.add_body(xform=X.transform((7.0, y, 0.5)))
+        b.add_shape_mesh(body, mesh=cube, scale=(scale, scale, scale))
+        expected.append((7.0, y, 0.3 * scale))
+    b.add_ground_plane()
+    model = b.finalize()
+    solver = si.SolverSemiImplicit(model, angular_damping=0.15, friction_smoothing=2.0)
+    pipe = oracle.CollisionPipeline(model, reduce_contacts=False)
+    contacts = pipe.contacts()
+    s0, s1, ctl = model.state(), model.state(), model.control()
+    dt = 1.0 / 60.0 / 30
+    for _ in range(120 * 30):
+        s0.clear_forces()
+        pipe.collide(s0, contacts)
+        solver.step(s0, s1, ctl, contacts, dt)
+        s0, s1 = s1, s0
+    q, qd = s0.body_q.numpy(), s0.body_qd.numpy()
+    assert np.isfinite(q).all() and np.isfinite(qd).all()
+    assert np.abs(qd[:, :3]).max() < 0.2 and np.abs(qd[:, 3:]).max() < 0.2
+    np.testing.assert_allclose(q[:, :3], np.array(expected), atol=0.25)
+    np.testing.assert_allclose(q[:, 3:], np.tile([0.0, 0.0, 0.0, 1.0], (model.body_count, 1)), atol=1e-1)
