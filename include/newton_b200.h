@@ -624,6 +624,55 @@ nb2_status nb2_actuator_param_gather(const int32_t* map, int32_t entries, const 
 nb2_status nb2_actuator_param_scatter(const int32_t* map, int32_t entries, int32_t dofs_per_world, const uint8_t* world_mask,
                                       const void* values, void* param, int32_t is_int, void* cuda_stream);
 
+/* --- joint-space impedance controllers (reference newton.controllers, controllers/impl/joint_impedance/) ------------------
+ * One WARP per robot, one launch per step:
+ *   acc = Kp (q_des - q) + Kd (qd_des - qd) [+ qdd];  tau = [M acc | acc] [+ g] [+ C qd];  joint_f[f_idx] = tau
+ * Robot r's dof i reads every flat input X through X_idx[dof_offsets[r] + i]; gains are [robot_count, max_dofs] and
+ * mass_matrix [robot_count, max_dofs, max_dofs].  Only the robot's dofs_per_robot[r] dofs are written.
+ * With `model` set (ControllerJointImpedance) the robots are the model's articulations, in order, and M, g and C qd come from the
+ * model itself: q and qd are gathered into state_joint_q / state_joint_qd, forward kinematics writes state_body_q /
+ * state_body_qd, and M / the two RNEA passes of nb2_eval_inverse_dynamics_passive run in shared memory (mass_matrix,
+ * gravity_force and coriolis_force and their index tables are then not read).  Without `model` the caller supplies them.
+ * Nothing is allocated and nothing synchronises the host. */
+typedef struct nb2_joint_impedance_desc {
+    int32_t robot_count;
+    int32_t max_dofs;                   /* row length of the gains and of mass_matrix */
+    int32_t use_gravity;                /* add g */
+    int32_t use_coriolis;               /* add C qd */
+    int32_t use_inertia;                /* premultiply acc by M */
+    int32_t has_qdd;                    /* add the qdd feedforward to acc */
+    const int32_t* dofs_per_robot;      /* [robot_count] */
+    const int32_t* dof_offsets;         /* [robot_count] start of each robot in the index tables */
+    const int32_t* joint_q_idx;         /* [sum dofs_per_robot] each */
+    const int32_t* joint_qd_idx;
+    const int32_t* joint_q_des_idx;
+    const int32_t* joint_qd_des_idx;
+    const int32_t* joint_qdd_idx;
+    const int32_t* gravity_force_idx;
+    const int32_t* coriolis_force_idx;
+    const int32_t* joint_f_idx;         /* distinct entries */
+    const float* joint_q;
+    const float* joint_qd;
+    const float* joint_q_des;
+    const float* joint_qd_des;
+    const float* joint_qdd;             /* has_qdd */
+    const float* gravity_force;         /* model-free with use_gravity */
+    const float* coriolis_force;        /* model-free with use_coriolis */
+    const float* mass_matrix;           /* model-free with use_inertia */
+    const float* stiffness;
+    const float* damping;
+    float* joint_f;
+    nb2_model* model;                   /* model-based: the controller's own model; NULL = model-free */
+    float* state_joint_q;               /* model-based: the controller's internal state */
+    float* state_joint_qd;
+    float* state_body_q;
+    float* state_body_qd;
+} nb2_joint_impedance_desc;
+
+/* ControllerJointImpedance.step / ControllerJointImpedanceModelFree.step (controllers/impl/joint_impedance/).  A model-based
+ * robot whose shared-memory scratch exceeds one CTA is refused with NB2_ERR_CAPACITY before anything is launched. */
+nb2_status nb2_joint_impedance_step(const nb2_joint_impedance_desc* desc, void* cuda_stream);
+
 /* --- inverse kinematics (reference newton.ik, sim/ik/) ----------------------------------------------------------------------
  * Batched Levenberg-Marquardt IK over one articulated model: `n_batch` independent rows (problems x seeds) share the model and
  * the objective list.  nb2_ik_solve runs every LM iteration of every row in ONE launch (a sub-warp group of lanes per row, all

@@ -15,5 +15,6 @@ from . import solvers  # noqa: F401,E402
 from . import selection  # noqa: F401,E402
 from . import sensors  # noqa: F401,E402
 from . import actuators  # noqa: F401,E402
+from . import controllers  # noqa: F401,E402
 from . import ik  # noqa: F401,E402
 from .geometry import intersect_ray  # noqa: F401,E402

@@ -272,6 +272,40 @@ class ActuatorStepDesc(C.Structure):
                 ("scratch", C.c_void_p), ("clamps", ActuatorClamp * ACTUATOR_MAX_CLAMPS)]
 
 
+class JointImpedanceDesc(C.Structure):
+    """``nb2_joint_impedance_desc``"""
+
+    _fields_ = [(n, C.c_int32) for n in ("robot_count", "max_dofs", "use_gravity", "use_coriolis", "use_inertia", "has_qdd")] + [
+        (n, C.c_void_p) for n in (
+            "dofs_per_robot", "dof_offsets", "joint_q_idx", "joint_qd_idx", "joint_q_des_idx", "joint_qd_des_idx", "joint_qdd_idx",
+            "gravity_force_idx", "coriolis_force_idx", "joint_f_idx", "joint_q", "joint_qd", "joint_q_des", "joint_qd_des", "joint_qdd",
+            "gravity_force", "coriolis_force", "mass_matrix", "stiffness", "damping", "joint_f", "model", "state_joint_q",
+            "state_joint_qd", "state_body_q", "state_body_qd")]
+
+
+class DescCache:
+    """Launch descriptors built once per combination of arrays: a call that reads and writes the very same tensors (same
+    objects, addresses and sizes) and passes the same ``key`` reuses the descriptor built and checked for the first one.  The
+    tensors and the ``keep`` objects stay referenced by their entry, so their ids cannot be reused while it lives."""
+
+    def __init__(self, capacity: int = 4):
+        self._entries: dict = {}
+        self._capacity = capacity
+
+    def __len__(self) -> int:
+        return len(self._entries)
+
+    def get(self, arrays: tuple, build, key: tuple = (), keep: tuple = ()):
+        """The descriptor for ``arrays`` (tensors or None), built by ``build()`` on a miss."""
+        k = (*key, *((id(a), a.data_ptr(), a.numel()) if a is not None else None for a in arrays))
+        hit = self._entries.get(k)
+        if hit is None:
+            if len(self._entries) >= self._capacity:
+                self._entries.clear()
+            hit = self._entries[k] = (build(), arrays, keep)
+        return hit[0]
+
+
 class FeatherstoneParams(C.Structure):
     _fields_ = [
         ("angular_damping", C.c_float),

@@ -30,6 +30,7 @@ EXPORTED_SYMBOLS = (
     "nb2_eval_jacobian", "nb2_eval_mass_matrix", "nb2_eval_inverse_dynamics_passive", "nb2_eval_inverse_dynamics_force",
     "nb2_sensor_contact_scratch_bytes", "nb2_sensor_contact_update", "nb2_raycast_refit", "nb2_intersect_ray",
     "nb2_camera_render", "nb2_actuator_step", "nb2_actuator_reset", "nb2_actuator_param_gather", "nb2_actuator_param_scatter",
+    "nb2_joint_impedance_step",
     "nb2_ik_solve", "nb2_ik_sample", "nb2_ik_select",
     "nb2_view_gather", "nb2_view_scatter", "nb2_view_articulation_mask", "nb2_last_error", "nb2_kernel_launch_count", "nb2_version",
     "nb2_peer_gather_handle_bytes", "nb2_peer_gather_create", "nb2_peer_gather_buffer", "nb2_peer_gather_stride", "nb2_peer_gather_export",
@@ -117,6 +118,8 @@ def lib():
         L.nb2_actuator_param_gather.restype = C.c_int
         L.nb2_actuator_param_scatter.argtypes = [P, C.c_int32, C.c_int32, P, P, P, C.c_int32, P]
         L.nb2_actuator_param_scatter.restype = C.c_int
+        L.nb2_joint_impedance_step.argtypes = [C.POINTER(_abi.JointImpedanceDesc), P]
+        L.nb2_joint_impedance_step.restype = C.c_int
         L.nb2_ik_solve.argtypes = [P, P, P, P, P, P, P, P, C.c_int32, C.c_float, C.c_int32, P, P]
         L.nb2_ik_solve.restype = C.c_int
         L.nb2_ik_sample.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, P, P, P, P, P, C.c_float, P, P, P]

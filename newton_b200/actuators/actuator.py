@@ -156,7 +156,7 @@ class Actuator:
         targets, counts = np.unique(eff, return_counts=True)
         self.has_duplicate_effort_indices = bool((counts > 1).any())
         self._dup = None
-        self._desc_cache: dict = {}
+        self._desc_cache = _abi.DescCache()
         if self.has_duplicate_effort_indices:
             order = np.argsort(eff, kind="stable").astype(np.int32)  # ascending actuator index inside each target
             start = np.concatenate([[0], np.cumsum(counts)]).astype(np.int32)
@@ -262,23 +262,16 @@ class Actuator:
              next_act_state: Actuator.State | None = None, dt: float | None = None) -> None:
         """One control step: delay read, controller, clamping, scatter-add into ``sim_control.<control_output_attr>``, and the
         delay buffers / PID integral of ``next_act_state``.  ``dt`` [s] is required for PID."""
-        # A descriptor is built and checked once per combination of arrays: a later call that reads and writes the very same
-        # tensors (same objects, addresses and sizes) reuses it.  The ping-pong of two actuator states keeps two entries.
+        # A descriptor is built and checked once per combination of arrays (_abi.DescCache).  The ping-pong of two actuator
+        # states keeps two entries.
         arrays = self._arrays_read(sim_state, sim_control, current_act_state, next_act_state)
         if not all(a is None or isinstance(a, torch.Tensor) for a in arrays):  # other array types are checked every call
             d = self._step_desc(sim_state, sim_control, current_act_state, next_act_state, dt)
             _call("step", self.device, C.byref(d))
             return
-        key = (dt, id(current_act_state), id(next_act_state),
-               *((id(a), a.data_ptr(), a.numel()) if a is not None else None for a in arrays))
-        hit = self._desc_cache.get(key)
-        if hit is None:
-            if len(self._desc_cache) >= 4:
-                self._desc_cache.clear()
-            # the states and arrays are kept with the entry, so their ids cannot be reused while it lives
-            d = self._step_desc(sim_state, sim_control, current_act_state, next_act_state, dt)
-            hit = self._desc_cache[key] = (d, arrays, current_act_state, next_act_state)
-        _call("step", self.device, C.byref(hit[0]))
+        d = self._desc_cache.get(arrays, lambda: self._step_desc(sim_state, sim_control, current_act_state, next_act_state, dt),
+                                 key=(dt, id(current_act_state), id(next_act_state)), keep=(current_act_state, next_act_state))
+        _call("step", self.device, C.byref(d))
 
     def _arrays_read(self, sim_state, sim_control, current_act_state, next_act_state) -> tuple:
         """Every tensor a step descriptor points at, in a fixed order (None where absent)."""

@@ -1146,6 +1146,45 @@ nb2_status nb2_actuator_param_scatter(const int32_t* map, int32_t entries, int32
                                  static_cast<cudaStream_t>(cuda_stream));
 }
 
+nb2_status nb2_joint_impedance_step(const nb2_joint_impedance_desc* desc, void* cuda_stream) {
+    if (!desc) {
+        set_error("nb2_joint_impedance_step: NULL descriptor");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    const nb2_joint_impedance_desc& d = *desc;
+    if (d.robot_count < 0 || (d.robot_count > 0 && d.max_dofs < 1)) {
+        set_error("nb2_joint_impedance_step: invalid robot_count or max_dofs");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    if (d.robot_count == 0) return NB2_OK;
+    if (!d.dofs_per_robot || !d.dof_offsets || !d.joint_q_idx || !d.joint_qd_idx || !d.joint_q_des_idx || !d.joint_qd_des_idx ||
+        !d.joint_f_idx || !d.joint_q || !d.joint_qd || !d.joint_q_des || !d.joint_qd_des || !d.stiffness || !d.damping || !d.joint_f ||
+        (d.has_qdd && (!d.joint_qdd_idx || !d.joint_qdd))) {
+        set_error("nb2_joint_impedance_step: NULL index table, input, gain or output array");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    if (!d.model && ((d.use_gravity && (!d.gravity_force_idx || !d.gravity_force)) ||
+                     (d.use_coriolis && (!d.coriolis_force_idx || !d.coriolis_force)) || (d.use_inertia && !d.mass_matrix))) {
+        set_error("nb2_joint_impedance_step: a model-free step needs the caller's array of every enabled dynamics term");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    if (d.model) {
+        const nb2_model* m = d.model;
+        if (!d.state_joint_q || !d.state_joint_qd || ((d.use_inertia || d.use_gravity || d.use_coriolis) && (!d.state_body_q || !d.state_body_qd))) {
+            set_error("nb2_joint_impedance_step: a model-based step needs the internal state's arrays");
+            return NB2_ERR_INVALID_ARGUMENT;
+        }
+        if (d.robot_count != m->dev.d.articulation_count || d.max_dofs < m->host.tree_max_dofs) {
+            set_error("nb2_joint_impedance_step: robot_count must equal the model's articulation count and max_dofs cover its largest "
+                      "articulation");
+            return NB2_ERR_INVALID_ARGUMENT;
+        }
+        DeviceGuard guard(m->device);
+        return launch_joint_impedance_step(d, static_cast<cudaStream_t>(cuda_stream));
+    }
+    return launch_joint_impedance_step(d, static_cast<cudaStream_t>(cuda_stream));
+}
+
 const char* nb2_last_error(void) { return g_last_error.c_str(); }
 int64_t nb2_kernel_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
 const char* nb2_version(void) { return "newton_b200 0.1 (sm_90a)"; }

@@ -531,6 +531,93 @@ __global__ void __launch_bounds__(32 * DYN_WARPS) eval_inverse_dynamics_force_ke
     for (int i = t.d0 + t.nd + lane; i < gap_end; i += 32) tau[i] = 0.0f;
 }
 
+// ---- joint-space impedance controllers (controllers/impl/joint_impedance/) ---------------------------------------------------
+// One warp per robot.  MODEL (ControllerJointImpedance): robot r is articulation r; its q / qd are gathered into shared memory and
+// the internal state, forward kinematics writes the internal body_q / body_qd, and M and the g / C qd passes are formed in shared
+// memory by the code of eval_inverse_dynamics_passive_kernel.  !MODEL (ControllerJointImpedanceModelFree): M, g and C qd are the
+// caller's.  The law's operation order (each operation rounded): acc = Kp (q_des - q) + Kd (qd_des - qd), acc = acc + qdd;
+// tau = sum_c M[i][c] acc[c] from +0 in column order (or acc), tau = tau + g, tau = tau + C qd.
+// Shared memory per warp: acc [ND], and for MODEL q, qd, g, C qd [ND], M [ND][ND] and the dynamics scratch (dyn_smem_words).
+__host__ __device__ inline size_t ji_smem_words(bool model, int NJ, int ND) {
+    return model ? size_t(5) * ND + size_t(ND) * ND + dyn_smem_words(NJ, ND) : size_t(ND);
+}
+
+template <bool MODEL>
+__global__ void __launch_bounds__(32 * DYN_WARPS) joint_impedance_kernel(const nb2_joint_impedance_desc p, DevModel M, int fk_levels, int NJ,
+                                                                        int ND) {
+    extern __shared__ float dyn_smem[];
+    const int r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;  // warp-uniform
+    if (r >= p.robot_count) return;
+    const int lane = threadIdx.x & 31;
+    float* acc = dyn_smem + (threadIdx.x >> 5) * ji_smem_words(MODEL, NJ, ND);
+    const int n = p.dofs_per_robot[r], off = p.dof_offsets[r];
+    const float* H = p.use_inertia ? p.mass_matrix + size_t(r) * p.max_dofs * p.max_dofs : nullptr;
+    int LD = p.max_dofs;
+    float *q = nullptr, *qd = nullptr, *g = nullptr, *c = nullptr;
+    if constexpr (MODEL) {
+        const nb2_model_desc& d = M.d;
+        q = acc + ND;
+        qd = q + ND;
+        g = qd + ND;
+        c = g + ND;
+        float* Hs = c + ND;
+        DynSmem s = dyn_carve(Hs + size_t(ND) * ND, NJ, ND);
+        const Art t = art_of(d, r);  // its dofs are [off, off + n): the host admits only articulations that tile the dofs in order
+        for (int i = lane; i < n; i += 32) {
+            q[i] = p.state_joint_q[off + i] = p.joint_q[p.joint_q_idx[off + i]];
+            qd[i] = p.state_joint_qd[off + i] = p.joint_qd[p.joint_qd_idx[off + i]];
+        }
+        __syncwarp();
+        if (p.use_inertia || p.use_gravity || p.use_coriolis) {
+            const float* jq = q - t.d0;  // indexed by model coordinate (= dof: revolute / prismatic / fixed joints only)
+            const float* jqd = qd - t.d0;
+            if (fk_levels) {
+                fk_walk_levels(d, M.joint_depth, r, jq, jqd, p.state_body_q, p.state_body_qd, 3);
+            } else {
+                if (lane == 0) fk_walk_serial(d, r, jq, jqd, p.state_body_q, p.state_body_qd, 3);
+                __syncwarp();
+            }
+            tree_tables(d, t, s);
+            __syncwarp();
+            if (p.use_inertia) {
+                jacobian_smem(d, p.state_body_q, jq, t, s, ND);
+                world_inertias(d, p.state_body_q, t, s);
+                __syncwarp();
+                mass_matrix_entries(t, s, s.J, ND, Hs, ND);
+                H = Hs;
+                LD = ND;
+            }
+            if (p.use_gravity) rnea_pass(d, p.state_body_q, jq, nullptr, true, t, s, false, g - t.d0);
+            if (p.use_coriolis) rnea_pass(d, p.state_body_q, jq, jqd, false, t, s, false, c - t.d0);
+            __syncwarp();
+        }
+    }
+    for (int i = lane; i < n; i += 32) {
+        const int k = off + i;
+        const float qi = MODEL ? q[i] : p.joint_q[p.joint_q_idx[k]];
+        const float qdi = MODEL ? qd[i] : p.joint_qd[p.joint_qd_idx[k]];
+        const size_t gi = size_t(r) * p.max_dofs + i;
+        float a = p.stiffness[gi] * (p.joint_q_des[p.joint_q_des_idx[k]] - qi) + p.damping[gi] * (p.joint_qd_des[p.joint_qd_des_idx[k]] - qdi);
+        if (p.has_qdd) a = a + p.joint_qdd[p.joint_qdd_idx[k]];
+        acc[i] = a;
+    }
+    __syncwarp();
+    for (int i = lane; i < n; i += 32) {
+        const int k = off + i;
+        float tau;
+        if (p.use_inertia) {
+            tau = 0.0f;
+            const float* Hi = H + size_t(i) * LD;
+            for (int col = 0; col < n; ++col) tau = tau + Hi[col] * acc[col];
+        } else {
+            tau = acc[i];
+        }
+        if (p.use_gravity) tau = tau + (MODEL ? g[i] : p.gravity_force[p.gravity_force_idx[k]]);
+        if (p.use_coriolis) tau = tau + (MODEL ? c[i] : p.coriolis_force[p.coriolis_force_idx[k]]);
+        p.joint_f[p.joint_f_idx[k]] = tau;
+    }
+}
+
 // Launch geometry shared by the four entry points: DYN_WARPS articulations per CTA, fewer when the per-warp shared memory
 // would not fit; an articulation whose scratch exceeds one CTA's shared memory is refused.
 template <typename K>
@@ -626,6 +713,29 @@ nb2_status launch_eval_inverse_dynamics_force(nb2_model* m, const float* body_q,
         return st;
     eval_inverse_dynamics_force_kernel<<<blocks, threads, smem, s>>>(m->dev, body_q, H, joint_qdd, coriolis_force, gravity_force, mask, joint_f,
                                                                      max_dofs, ND);
+    count_launch();
+    NB2_CUDA_CHECK(cudaGetLastError());
+    return NB2_OK;
+}
+
+nb2_status launch_joint_impedance_step(const nb2_joint_impedance_desc& p, cudaStream_t s) {
+    if (p.robot_count == 0) return NB2_OK;
+    const char* what = "nb2_joint_impedance_step";
+    int blocks, threads;
+    size_t smem;
+    nb2_status st;
+    if (p.model) {
+        const nb2_model* m = p.model;
+        const int NJ = m->host.tree_max_joints, ND = m->host.tree_max_dofs > 0 ? m->host.tree_max_dofs : 1;
+        if ((st = dyn_launch_config(joint_impedance_kernel<true>, what, ji_smem_words(true, NJ, ND), p.robot_count, blocks, threads, smem)))
+            return st;
+        joint_impedance_kernel<true><<<blocks, threads, smem, s>>>(p, m->dev, m->host.fk_levels ? 1 : 0, NJ, ND);
+    } else {
+        if ((st = dyn_launch_config(joint_impedance_kernel<false>, what, ji_smem_words(false, 0, p.max_dofs), p.robot_count, blocks, threads,
+                                    smem)))
+            return st;
+        joint_impedance_kernel<false><<<blocks, threads, smem, s>>>(p, DevModel{}, 0, 0, p.max_dofs);
+    }
     count_launch();
     NB2_CUDA_CHECK(cudaGetLastError());
     return NB2_OK;

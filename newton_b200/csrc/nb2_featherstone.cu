@@ -1027,26 +1027,15 @@ __device__ __forceinline__ int fk_articulation(const nb2_model_desc& d, int item
     return a;
 }
 
-// One WARP per articulation, joints of equal tree depth in parallel (lane = joint), depth levels in order with __syncwarp()
-// between them (it orders the lanes' global writes and reads): a 13-joint quadruped takes 4 dependent steps instead of 13.
-// Every joint runs exactly the arithmetic of the serial walk on the same parent values, so the results are bit-identical to it.
-// Requires parent-before-child joint order and one driving joint per body (nb2_model::fk_levels, checked at model creation).
+// One WARP per articulation walking its tree level by level (fk_walk_levels, nb2_joint.cuh): a 13-joint quadruped takes 4
+// dependent steps instead of 13.  Requires nb2_model::fk_levels, checked at model creation.
 __global__ void __launch_bounds__(128) eval_fk_levels_kernel(DevModel M, const float* __restrict__ joint_q, const float* __restrict__ joint_qd,
                                                              float* body_q, float* body_qd, const uint8_t* __restrict__ mask,
                                                              const int* __restrict__ indices, int count, int body_flag_filter) {
     const nb2_model_desc& d = M.d;
-    const int lane = threadIdx.x & 31;
     const int a = fk_articulation(d, (blockIdx.x * blockDim.x + threadIdx.x) >> 5, count, mask, indices);  // warp-uniform
     if (a < 0) return;
-    const int j0 = d.articulation_start[a], j1 = d.articulation_start[a + 1];
-    int deepest = 0;
-    for (int i = j0 + lane; i < j1; i += 32) deepest = max(deepest, M.joint_depth[i]);
-    for (int o = 16; o > 0; o >>= 1) deepest = max(deepest, __shfl_xor_sync(0xffffffffu, deepest, o));
-    for (int level = 0; level <= deepest; ++level) {
-        for (int i = j0 + lane; i < j1; i += 32)
-            if (M.joint_depth[i] == level && d.joint_articulation[i] != -1) fk_joint(d, i, joint_q, joint_qd, body_q, body_qd, body_flag_filter);
-        __syncwarp();
-    }
+    fk_walk_levels(d, M.joint_depth, a, joint_q, joint_qd, body_q, body_qd, body_flag_filter);
 }
 
 // Fallback for models whose joint order the level schedule cannot honour: one thread walks one articulation in joint order.
@@ -1056,8 +1045,7 @@ __global__ void __launch_bounds__(128) eval_fk_kernel(DevModel M, const float* _
     const nb2_model_desc& d = M.d;
     const int a = fk_articulation(d, blockIdx.x * blockDim.x + threadIdx.x, count, mask, indices);
     if (a < 0) return;
-    for (int i = d.articulation_start[a]; i < d.articulation_start[a + 1]; ++i)
-        if (d.joint_articulation[i] != -1) fk_joint(d, i, joint_q, joint_qd, body_q, body_qd, body_flag_filter);
+    fk_walk_serial(d, a, joint_q, joint_qd, body_q, body_qd, body_flag_filter);
 }
 
 nb2_status launch_eval_fk(nb2_model* m, const float* joint_q, const float* joint_qd, float* body_q, float* body_qd, cudaStream_t s,

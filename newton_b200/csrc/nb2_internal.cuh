@@ -258,6 +258,7 @@ nb2_status launch_intersect_ray(const nb2_raycast_view& v, int ray_count, const 
                                 bool enable_global_world, float* out_dist, int* out_shape_id, float* out_normal, cudaStream_t s);
 nb2_status launch_camera_render(const nb2_raycast_view& v, const nb2_camera_desc& c, cudaStream_t s);
 nb2_status launch_actuator_step(const nb2_actuator_step_desc& desc, cudaStream_t s);
+nb2_status launch_joint_impedance_step(const nb2_joint_impedance_desc& desc, cudaStream_t s);
 nb2_status launch_actuator_reset(int count, int buf_depth, const uint8_t* mask, float* buf_pos, float* buf_vel, float* buf_act,
                                  int* num_pushes, int* write_idx, float* integral, cudaStream_t s);
 nb2_status launch_actuator_param(bool gather, const int* map, int entries, int dofs_per_world, const uint8_t* world_mask, const void* src,

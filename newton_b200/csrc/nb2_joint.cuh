@@ -98,6 +98,31 @@ __device__ __forceinline__ void fk_joint(const nb2_model_desc& d, int i, const f
     st6(body_qd + 6 * child, S6(v_com, w_o));
 }
 
+// Articulation a's joints [j0, j1) walked by one WARP, joints of equal tree depth in parallel (lane = joint), depth levels in
+// order with __syncwarp() between them (it orders the lanes' global writes and reads).  Every joint runs exactly the arithmetic
+// of the serial walk on the same parent values, so the results are bit-identical to it.  Requires parent-before-child joint
+// order and one driving joint per body (nb2_model::fk_levels).
+__device__ __forceinline__ void fk_walk_levels(const nb2_model_desc& d, const int* __restrict__ joint_depth, int a, const float* joint_q,
+                                               const float* joint_qd, float* body_q, float* body_qd, int body_flag_filter) {
+    const int lane = threadIdx.x & 31;
+    const int j0 = d.articulation_start[a], j1 = d.articulation_start[a + 1];
+    int deepest = 0;
+    for (int i = j0 + lane; i < j1; i += 32) deepest = max(deepest, joint_depth[i]);
+    for (int o = 16; o > 0; o >>= 1) deepest = max(deepest, __shfl_xor_sync(0xffffffffu, deepest, o));
+    for (int level = 0; level <= deepest; ++level) {
+        for (int i = j0 + lane; i < j1; i += 32)
+            if (joint_depth[i] == level && d.joint_articulation[i] != -1) fk_joint(d, i, joint_q, joint_qd, body_q, body_qd, body_flag_filter);
+        __syncwarp();
+    }
+}
+
+// The serial walk in joint order, by one thread: models whose joint order the level schedule cannot honour.
+__device__ __forceinline__ void fk_walk_serial(const nb2_model_desc& d, int a, const float* joint_q, const float* joint_qd, float* body_q,
+                                               float* body_qd, int body_flag_filter) {
+    for (int i = d.articulation_start[a]; i < d.articulation_start[a + 1]; ++i)
+        if (d.joint_articulation[i] != -1) fk_joint(d, i, joint_q, joint_qd, body_q, body_qd, body_flag_filter);
+}
+
 // jcalc_motion_subspace / write_free_distance_motion_subspace (sim/articulation.py:934-1069) of joint j: its columns S[6 * k ..]
 // (k = dof within the joint, zeroed first) from the parent anchor X_wpj = body_q[parent] * joint_X_p and the world COM xc of its
 // child (read by FREE / DISTANCE only).  ROD columns stay zero (:1011-1013).

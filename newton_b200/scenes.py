@@ -564,8 +564,14 @@ PANDA_HOME = (0.0, -0.785, 0.0, -2.356, 0.0, 1.571, 0.785, 0.02, 0.02)
 
 
 def panda_arm_model(device="cpu"):
-    """One Panda-class arm for inverse kinematics: 10 bodies / 10 joints (7 revolute, 1 fixed hand, 2 prismatic fingers), 9 dofs,
-    joint j driving body j (the layout the analytic IK mode needs).  Body 7 is the hand; ``joint_q`` starts at ``PANDA_HOME``."""
+    """One Panda-class arm for inverse kinematics (:func:`panda_arm_builder`), finalized with its bodies placed at
+    ``PANDA_HOME``."""
+    return _finish(panda_arm_builder(), device)
+
+
+def panda_arm_builder() -> ModelBuilder:
+    """One Panda-class arm: 10 bodies / 10 joints (7 revolute, 1 fixed hand, 2 prismatic fingers), 9 dofs, joint j driving body
+    j (the layout the analytic IK mode needs).  Body 7 is the hand; ``joint_q`` starts at ``PANDA_HOME``."""
     b = ModelBuilder()
     inertia = np.eye(3) * 0.01
     parent = -1
@@ -585,4 +591,26 @@ def panda_arm_model(device="cpu"):
                               limit_upper=0.04, label=f"panda/finger_joint{1 if side > 0 else 2}")
     b.add_articulation(list(range(b.joint_count)), label="panda")
     b.joint_q = list(PANDA_HOME)
-    return _finish(b, device)
+    return b
+
+
+# ---- joint-impedance control workloads (scripts/controller_bench.py, tests/test_*controllers.py) -------------------------------
+def pendulum_link_builder(mass: float = 1.0, length: float = 0.5, inertia: float = 0.01) -> ModelBuilder:
+    """One revolute link hanging from the world: axis y, COM ``length`` below the joint at ``q = 0`` (so ``g(q) = m g l sin q``,
+    ``M = I + m l^2``)."""
+    b = ModelBuilder()
+    link = b.add_link(mass=mass, com=(0.0, 0.0, -length), inertia=np.eye(3) * inertia, label="pendulum/link")
+    b.add_joint_revolute(-1, link, axis=(0.0, 1.0, 0.0), label="pendulum/joint")
+    b.add_articulation([0], label="pendulum")
+    return b
+
+
+def impedance_fleet_builder(robot_count: int, kinds=("panda",)) -> ModelBuilder:
+    """``robot_count`` fixed-base robots, one world each, cycling through ``kinds``: "panda" (:func:`panda_arm_builder`, 9 dofs),
+    "ant" (fixed-base :func:`ant_builder`, 8 dofs) and "pendulum" (:func:`pendulum_link_builder`, 1 dof)."""
+    make = {"panda": panda_arm_builder, "ant": lambda: ant_builder(floating=False), "pendulum": pendulum_link_builder}
+    robots = {k: make[k]() for k in kinds}
+    scene = ModelBuilder()
+    for r in range(robot_count):
+        scene.add_world(robots[kinds[r % len(kinds)]])
+    return scene
