@@ -217,13 +217,14 @@ def test_generated_joint_states(oracle_si):
 
 
 # ---- generated contact states ------------------------------------------------------------------------------------------------
-def contact_scene(seed, worlds=2, bodies=4, per_pair=4):
+def contact_scene(seed, worlds=2, bodies=4, per_pair=4, depth=(0.005, 0.05), speed=(0.02, 4.0)):
     """Jointless bodies (a kinematic one and one with inv_mass = 0 among them), static shapes in each world and the global ground,
     per-world gravity, and a hand-written Contacts buffer whose separations are placed on purpose: penetrating, in the adhesion
     band 0 <= d < ka and beyond ka, for dynamic-dynamic, dynamic-static, one-sided (shape -1 on either side) and same-shape rows,
     with random margins and velocities spanning the friction smoothing widths.  ``per_pair`` = 4 writes two penetrating rows, one
     in the band and one beyond per shape pair (100 per world); 2 writes one penetrating row and one in the band or beyond (50 per
-    world, within the 70 contact slots the native solvers give such a world: 5 per candidate shape pair)."""
+    world, within the 70 contact slots the native solvers give such a world: 5 per candidate shape pair).  ``depth`` is the range
+    of penetration depths and ``speed`` the range of twist scales the bodies draw."""
     from newton_b200.sim.model import Contacts
 
     rng = np.random.default_rng(seed)
@@ -245,7 +246,7 @@ def contact_scene(seed, worlds=2, bodies=4, per_pair=4):
     b.add_ground_plane(cfg=cfg())
     model = b.finalize()
     n = model.body_count
-    qd = rng.normal(size=(n, 6)) * np.exp(rng.uniform(np.log(0.02), np.log(4.0), (n, 1)))
+    qd = rng.normal(size=(n, 6)) * np.exp(rng.uniform(np.log(speed[0]), np.log(speed[1]), (n, 1)))
     model.body_qd.copy_(torch.from_numpy(qd.astype(np.float32)))
     shape_body, shape_world = model.shape_body.numpy(), model.shape_world.numpy()
     body_q = model.body_q.numpy().astype(np.float64)
@@ -276,7 +277,7 @@ def contact_scene(seed, worlds=2, bodies=4, per_pair=4):
             for kind in ("pen", "pen", "band", "beyond") if per_pair == 4 else ("pen", ("band", "beyond")[j % 2]):
                 present = [s for s in (sa, sb) if s >= 0]
                 k = float(np.mean(ka[present])) if present else 0.0
-                d = {"pen": -rng.uniform(0.005, 0.05), "band": k * rng.uniform(0.2, 0.8), "beyond": k + rng.uniform(0.003, 0.02)}[kind]
+                d = {"pen": -rng.uniform(*depth), "band": k * rng.uniform(0.2, 0.8), "beyond": k + rng.uniform(0.003, 0.02)}[kind]
                 nrm = rng.normal(size=3)
                 nrm /= np.linalg.norm(nrm)
                 n_ = -nrm
