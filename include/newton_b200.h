@@ -550,9 +550,51 @@ nb2_status nb2_camera_render(const nb2_raycast_view* view, const nb2_camera_desc
  * delay buffer and PID state of the next state.  Index arrays are int32 (the reference's uint32 values).  The host
  * (newton_b200.actuators.Actuator) fills the descriptor; the library keeps no per-actuator state, allocates nothing and does
  * not synchronise, so a step can be captured into a CUDA graph.  Strict fp32 in the reference's operation order. */
-enum { NB2_ACT_PD = 0, NB2_ACT_PID = 1 };
+enum { NB2_ACT_PD = 0, NB2_ACT_PID = 1, NB2_ACT_MLP = 2, NB2_ACT_LSTM = 3 };
 enum { NB2_CLAMP_MAX_EFFORT = 1, NB2_CLAMP_DC_MOTOR = 2, NB2_CLAMP_POSITION_BASED = 3 };
 enum { NB2_ACTUATOR_MAX_CLAMPS = 8, NB2_ACTUATOR_MAX_LOOKUP = 2048 };
+
+/* Learned actuator networks (reference ControllerNeuralMLP / ControllerNeuralLSTM, Torch checkpoints).  One thread per actuator
+ * owns whole dot products; a CTA of NB2_NET_TILE actuators stages the group's packed weights, its lookup tables and its
+ * activation scratch in shared memory, which must fit NB2_ACTUATOR_SMEM_MAX bytes (else NB2_ERR_CAPACITY):
+ *   4 * (round_up(weight_count, 4) + 2 * lookup entries + scratch) bytes, with scratch
+ *   MLP:  2 * max(widths) * NB2_NET_TILE floats        LSTM: 4 * hidden_size * (NB2_NET_TILE + 1) floats.
+ *
+ * Packed weights (float32, row-major [out][in]):
+ *   MLP, per Linear layer l: W_l [widths[l + 1]][widths[l]], then b_l [widths[l + 1]] when has_bias[l].
+ *   LSTM, per layer l: W_ih [4H][in_l] (in_0 = 2, else H), W_hh [4H][H], then b_ih [4H], b_hh [4H] when has_bias[0];
+ *         then the head W [1][H] and, when has_bias[1], b [1].  Gate rows in torch's order i, f, g, o.
+ *
+ * Arithmetic contract (the CPU oracle follows it too; the strict library rounds every operation to fp32, no contraction):
+ *   Linear row r:  acc = W[r,0] x[0];  acc = acc + W[r,k] x[k] for k = 1 .. K-1;  y = acc + b[r]  (y = acc without bias).
+ *   LSTM gate row r:  a = (dot(W_ih[r], x) + b_ih[r]) + (dot(W_hh[r], h) + b_hh[r]), each dot as above;
+ *                     c' = (f c) + (i g),  h' = o tanh(c').
+ *   sigmoid(a) = (float)(1 / (1 + exp(-(double)a)));  tanh(a) = (float)tanh((double)a);
+ *   ELU(a) = a > 0 ? a : (float)(alpha expm1((double)a)) with alpha as double;  softsign(a) = a / (1 + |a|);
+ *   ReLU(a) = a < 0 ? 0 : a (NaN passes through).  The fast library evaluates the same formulas in fp32 with contraction.
+ *   Scales are fp32: MLP input = (k == 0 ? e : history[k - 1]) * scale, LSTM input = [e * pos_scale, v * vel_scale],
+ *   computed = net(x) * effort_scale, where e = (delayed) target position - position and v = the joint velocity. */
+enum { NB2_NET_NONE = 0, NB2_NET_RELU = 1, NB2_NET_ELU = 2, NB2_NET_TANH = 3, NB2_NET_SIGMOID = 4, NB2_NET_SOFTSIGN = 5 };
+enum { NB2_NET_MAX_LAYERS = 16, NB2_NET_MAX_INPUTS = 32, NB2_NET_TILE = 128, NB2_ACTUATOR_SMEM_MAX = 227 * 1024 };
+
+typedef struct nb2_actuator_network {
+    int32_t layer_count;                       /* MLP: Linear layers; LSTM: LSTM layers (the head is extra) */
+    int32_t widths[NB2_NET_MAX_LAYERS + 1];    /* MLP: in, hidden ..., 1; LSTM: widths[0] = 2, widths[1] = hidden_size */
+    int32_t activation[NB2_NET_MAX_LAYERS];    /* MLP: NB2_NET_* after layer l (NONE after the last) */
+    float alpha[NB2_NET_MAX_LAYERS];           /* MLP: ELU alpha of layer l */
+    int32_t has_bias[NB2_NET_MAX_LAYERS];      /* MLP: per layer; LSTM: [0] the LSTM, [1] the head */
+    int32_t weight_count;                      /* floats in weights */
+    const float* weights;                      /* packed, on the device */
+    int32_t input_count;                       /* MLP: len(input_idx) */
+    int32_t input_idx[NB2_NET_MAX_INPUTS];     /* MLP: history entries, 0 = the current step */
+    int32_t vel_first;                         /* MLP: input_order "vel_pos" */
+    int32_t history_length;                    /* MLP: max(input_idx) + 1; the history arrays are [history_length, N] */
+    float pos_scale, vel_scale, effort_scale;
+    const float* state0_in;   /* MLP: pos_error_history; LSTM: hidden [L, N, H] */
+    const float* state1_in;   /* MLP: vel_history;       LSTM: cell [L, N, H] */
+    float* state0_out;        /* the next state's arrays, distinct from the current state's */
+    float* state1_out;
+} nb2_actuator_network;
 
 typedef struct nb2_actuator_clamp {
     int32_t kind;          /* NB2_CLAMP_* */
@@ -605,6 +647,9 @@ typedef struct nb2_actuator_step_desc {
     const int32_t* dup_actuator;
     float* scratch;
     nb2_actuator_clamp clamps[NB2_ACTUATOR_MAX_CLAMPS];
+    /* NB2_ACT_MLP / NB2_ACT_LSTM: the network and its state (kp, kd and const_effort are unused); NULL otherwise.  The
+     * delay still buffers the target velocity and feedforward, which the networks do not read. */
+    const nb2_actuator_network* network;
 } nb2_actuator_step_desc;
 
 /* Reference Actuator.step (actuators/actuator.py:204-332) for one group. */
@@ -615,6 +660,12 @@ nb2_status nb2_actuator_step(const nb2_actuator_step_desc* desc, void* cuda_stre
  * may be NULL (buf_depth 0 for no delay state). */
 nb2_status nb2_actuator_reset(int32_t count, int32_t buf_depth, const uint8_t* mask, float* buf_pos, float* buf_vel, float* buf_act,
                               int32_t* num_pushes, int32_t* write_idx, float* integral, void* cuda_stream);
+
+/* ControllerNeuralMLP.State / ControllerNeuralLSTM.State reset: zeroes element (r, i, j) of the two [rows, count, width]
+ * arrays a and b (MLP histories: rows = history_length, width 1; LSTM hidden / cell: rows = num_layers, width = hidden_size)
+ * for every actuator i (mask NULL) or those whose mask entry is set. */
+nb2_status nb2_actuator_network_reset(int32_t count, int32_t rows, int32_t width, const uint8_t* mask, float* a, float* b,
+                                      void* cuda_stream);
 
 /* ArticulationView actuator parameters: `map` [world_count * dofs_per_world] holds the parameter index of each view dof, or -1.
  * gather writes values[k] = map[k] >= 0 ? param[map[k]] : 0; scatter writes param[map[k]] = values[k] for mapped entries of

@@ -248,7 +248,9 @@ class CameraDesc(C.Structure):
                 ("clear_depth", C.c_float), ("clear_shape_index", C.c_uint32), ("clear_normal", C.c_float * 3)]
 
 
-ACT_PD, ACT_PID = 0, 1  # NB2_ACT_*
+ACT_PD, ACT_PID, ACT_MLP, ACT_LSTM = 0, 1, 2, 3  # NB2_ACT_*
+NET_NONE, NET_RELU, NET_ELU, NET_TANH, NET_SIGMOID, NET_SOFTSIGN = 0, 1, 2, 3, 4, 5  # NB2_NET_*
+NET_MAX_LAYERS, NET_MAX_INPUTS, NET_TILE, ACTUATOR_SMEM_MAX = 16, 32, 128, 227 * 1024
 CLAMP_MAX_EFFORT, CLAMP_DC_MOTOR, CLAMP_POSITION_BASED = 1, 2, 3  # NB2_CLAMP_*
 ACTUATOR_MAX_CLAMPS, ACTUATOR_MAX_LOOKUP = 8, 2048  # NB2_ACTUATOR_MAX_*
 
@@ -257,6 +259,16 @@ class ActuatorClamp(C.Structure):
     """``nb2_actuator_clamp``"""
 
     _fields_ = [("kind", C.c_int32), ("lookup_size", C.c_int32), ("p0", C.c_void_p), ("p1", C.c_void_p), ("p2", C.c_void_p)]
+
+
+class ActuatorNetwork(C.Structure):
+    """``nb2_actuator_network``"""
+
+    _fields_ = [("layer_count", C.c_int32), ("widths", C.c_int32 * (NET_MAX_LAYERS + 1)), ("activation", C.c_int32 * NET_MAX_LAYERS),
+                ("alpha", C.c_float * NET_MAX_LAYERS), ("has_bias", C.c_int32 * NET_MAX_LAYERS), ("weight_count", C.c_int32),
+                ("weights", C.c_void_p), ("input_count", C.c_int32), ("input_idx", C.c_int32 * NET_MAX_INPUTS), ("vel_first", C.c_int32),
+                ("history_length", C.c_int32), ("pos_scale", C.c_float), ("vel_scale", C.c_float), ("effort_scale", C.c_float),
+                ("state0_in", C.c_void_p), ("state1_in", C.c_void_p), ("state0_out", C.c_void_p), ("state1_out", C.c_void_p)]
 
 
 class ActuatorStepDesc(C.Structure):
@@ -269,7 +281,7 @@ class ActuatorStepDesc(C.Structure):
                     "delay_steps", "buf_pos_in", "buf_vel_in", "buf_act_in", "num_pushes_in", "write_idx_in", "buf_pos_out",
                     "buf_vel_out", "buf_act_out", "num_pushes_out", "write_idx_out", "output", "computed_output")] + [
                 ("dup_target_count", C.c_int32), ("dup_target", C.c_void_p), ("dup_start", C.c_void_p), ("dup_actuator", C.c_void_p),
-                ("scratch", C.c_void_p), ("clamps", ActuatorClamp * ACTUATOR_MAX_CLAMPS)]
+                ("scratch", C.c_void_p), ("clamps", ActuatorClamp * ACTUATOR_MAX_CLAMPS), ("network", C.POINTER(ActuatorNetwork))]
 
 
 class JointImpedanceDesc(C.Structure):

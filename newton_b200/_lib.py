@@ -29,7 +29,7 @@ EXPORTED_SYMBOLS = (
     "nb2_xpbd_step", "nb2_xpbd_update_contacts", "nb2_integrate_bodies", "nb2_featherstone_step", "nb2_semi_implicit_step", "nb2_eval_fk", "nb2_eval_ik", "nb2_eval_fk_masked",
     "nb2_eval_jacobian", "nb2_eval_mass_matrix", "nb2_eval_inverse_dynamics_passive", "nb2_eval_inverse_dynamics_force",
     "nb2_sensor_contact_scratch_bytes", "nb2_sensor_contact_update", "nb2_raycast_refit", "nb2_intersect_ray",
-    "nb2_camera_render", "nb2_actuator_step", "nb2_actuator_reset", "nb2_actuator_param_gather", "nb2_actuator_param_scatter",
+    "nb2_camera_render", "nb2_actuator_step", "nb2_actuator_reset", "nb2_actuator_network_reset", "nb2_actuator_param_gather", "nb2_actuator_param_scatter",
     "nb2_joint_impedance_step",
     "nb2_ik_solve", "nb2_ik_sample", "nb2_ik_select",
     "nb2_view_gather", "nb2_view_scatter", "nb2_view_articulation_mask", "nb2_last_error", "nb2_kernel_launch_count", "nb2_version",
@@ -114,6 +114,8 @@ def lib():
         L.nb2_actuator_step.restype = C.c_int
         L.nb2_actuator_reset.argtypes = [C.c_int32, C.c_int32, P, P, P, P, P, P, P, P]
         L.nb2_actuator_reset.restype = C.c_int
+        L.nb2_actuator_network_reset.argtypes = [C.c_int32, C.c_int32, C.c_int32, P, P, P, P]
+        L.nb2_actuator_network_reset.restype = C.c_int
         L.nb2_actuator_param_gather.argtypes = [P, C.c_int32, P, P, C.c_int32, P]
         L.nb2_actuator_param_gather.restype = C.c_int
         L.nb2_actuator_param_scatter.argtypes = [P, C.c_int32, C.c_int32, P, P, P, C.c_int32, P]

@@ -1,5 +1,5 @@
-"""Actuators (reference ``newton.actuators``): PD / PID control laws, command delay and effort clamping composed into an
-:class:`Actuator`, stepped on the GPU by one fused kernel per actuator group.  ``ModelBuilder.add_actuator`` groups
+"""Actuators (reference ``newton.actuators``): PD / PID control laws and learned MLP / LSTM actuator networks, command delay
+and effort clamping composed into an :class:`Actuator`, stepped on the GPU by one fused kernel per actuator group.  ``ModelBuilder.add_actuator`` groups
 compatible actuators into ``Model.actuators`` at ``finalize``."""
 
 from .actuator import Actuator
@@ -13,6 +13,7 @@ from .components import (
     ControllerPID,
     Delay,
 )
+from .neural import ControllerNeuralLSTM, ControllerNeuralMLP, load_metadata
 
 __all__ = [
     "Actuator",
@@ -21,7 +22,10 @@ __all__ = [
     "ClampingMaxEffort",
     "ClampingPositionBased",
     "Controller",
+    "ControllerNeuralLSTM",
+    "ControllerNeuralMLP",
     "ControllerPD",
     "ControllerPID",
     "Delay",
+    "load_metadata",
 ]

@@ -20,6 +20,7 @@ from .components import (
     ControllerPID,
     Delay,
 )
+from .neural import NEURAL_CONTROLLERS
 
 def _call(name: str, device, *args) -> None:
     """``nb2_actuator_<name>(*args, stream)`` on ``device``'s current stream: the one place the actuators launch."""
@@ -92,7 +93,8 @@ class Actuator:
 
         Args:
             indices: dof indices into velocity-shaped arrays (velocities, velocity targets, feedforward, effort output), ``(N,)``.
-            controller: :class:`ControllerPD` or :class:`ControllerPID`.
+            controller: :class:`ControllerPD`, :class:`ControllerPID`, :class:`ControllerNeuralMLP` or
+                :class:`ControllerNeuralLSTM`.
             delay: optional :class:`Delay`.
             clamping: list of clampings applied in order after the controller.
             pos_indices: indices into coordinate-shaped arrays (``state.joint_q``); default *indices*.
@@ -119,8 +121,9 @@ class Actuator:
         self.controller = controller
         self.delay = delay
         self.clamping = list(clamping or [])
-        if not isinstance(controller, (ControllerPD, ControllerPID)):
-            raise NotImplementedError(f"{type(controller).__name__}: only ControllerPD and ControllerPID are supported")
+        if not isinstance(controller, (ControllerPD, ControllerPID, *NEURAL_CONTROLLERS)):
+            raise NotImplementedError(f"{type(controller).__name__}: only ControllerPD, ControllerPID, ControllerNeuralMLP and "
+                                      f"ControllerNeuralLSTM are supported")
         for c in self.clamping:
             if not isinstance(c, (ClampingMaxEffort, ClampingDCMotor, ClampingPositionBased)):
                 raise NotImplementedError(f"{type(c).__name__}: unsupported clamping")
@@ -140,8 +143,17 @@ class Actuator:
         for component in (controller, delay, *self.clamping):
             if component is not None:
                 component.finalize(self.device, self.num_actuators)
-        if sum(c.lookup_size for c in self.clamping if isinstance(c, ClampingPositionBased)) > _abi.ACTUATOR_MAX_LOOKUP:
+        lookup = sum(c.lookup_size for c in self.clamping if isinstance(c, ClampingPositionBased))
+        if lookup > _abi.ACTUATOR_MAX_LOOKUP:
             raise ValueError(f"the lookup tables of one actuator hold at most {_abi.ACTUATOR_MAX_LOOKUP} entries in all")
+        if isinstance(controller, NEURAL_CONTROLLERS) and controller.smem_bytes(lookup) > _abi.ACTUATOR_SMEM_MAX:
+            from .. import _lib
+
+            raise _lib.Nb2Error(
+                f"{type(controller).__name__}('{controller.model_path}'): NB2_ERR_CAPACITY: the fused step stages the network in "
+                f"shared memory and needs {controller.smem_bytes(lookup)} bytes per CTA ({4 * controller.weights.numel()} of "
+                f"weights, {4 * controller._scratch_floats()} of activation scratch for {_abi.NET_TILE} actuators, "
+                f"{8 * lookup} of lookup tables); one CTA holds {_abi.ACTUATOR_SMEM_MAX}")
 
         # host-side tables, built once: the largest index of each index array (the element counts step() checks) and, for
         # effort indices that repeat, the per-target lists of the ordered second pass
@@ -188,12 +200,13 @@ class Actuator:
         if self.is_stateful() and current_act_state is next_act_state:
             raise ValueError("current_act_state and next_act_state must be different states (the step reads one and writes the other)")
         pid = isinstance(self.controller, ControllerPID)
+        neural = isinstance(self.controller, NEURAL_CONTROLLERS)
         if pid and dt is None:
             raise ValueError("ControllerPID needs dt")
         n, dev, P = self.num_actuators, self.device, _abi.ptr
         d = _abi.ActuatorStepDesc()
         d.count = n
-        d.controller = _abi.ACT_PID if pid else _abi.ACT_PD
+        d.controller = self.controller._KIND if neural else _abi.ACT_PID if pid else _abi.ACT_PD
         d.dt = float(dt) if dt is not None else 0.0
         d.indices = P(self.indices, "i32", dev, n, "indices")
         d.pos_indices = P(self.pos_indices, "i32", dev, n, "pos_indices")
@@ -218,9 +231,13 @@ class Actuator:
         if d.output in inputs or (d.computed_output is not None and d.computed_output in inputs):
             raise ValueError("the actuator's output arrays must not be any of its input arrays")
         c = self.controller
-        d.kp = P(c.kp, "f32", dev, n, "kp")
-        d.kd = P(c.kd, "f32", dev, n, "kd")
-        d.const_effort = P(c.const_effort, "f32", dev, n, "const_effort")
+        if neural:
+            net = c._network_desc(current_act_state.controller_state, next_act_state.controller_state)
+            d.network = C.pointer(net)  # the pointer keeps the structure alive with the descriptor
+        else:
+            d.kp = P(c.kp, "f32", dev, n, "kp")
+            d.kd = P(c.kd, "f32", dev, n, "kd")
+            d.const_effort = P(c.const_effort, "f32", dev, n, "const_effort")
         if pid:
             d.ki = P(c.ki, "f32", dev, n, "ki")
             d.integral_max = P(c.integral_max, "f32", dev, n, "integral_max")
@@ -284,10 +301,12 @@ class Actuator:
                 out.extend(getattr(component, n) for n in component._ARRAYS)
                 if isinstance(component, ClampingPositionBased):
                     out += [component.lookup_positions, component.lookup_efforts]
+        if isinstance(self.controller, NEURAL_CONTROLLERS):
+            out.append(self.controller.weights)
         for st in (current_act_state, next_act_state):
             ds = st.delay_state if st is not None else None
             cs = st.controller_state if st is not None else None
-            out += [getattr(cs, "integral", None)] + ([ds.buffer_pos, ds.buffer_vel, ds.buffer_act, ds.num_pushes, ds.write_idx]
+            out += [getattr(cs, n, None) for n in ("integral", "pos_error_history", "vel_history", "hidden", "cell")] + ([ds.buffer_pos, ds.buffer_vel, ds.buffer_act, ds.num_pushes, ds.write_idx]
                                                        if ds is not None else [None] * 5)
         return tuple(out)
 

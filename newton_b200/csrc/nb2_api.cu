@@ -1066,7 +1066,7 @@ nb2_status nb2_actuator_step(const nb2_actuator_step_desc* desc, void* cuda_stre
     }
     const nb2_actuator_step_desc& d = *desc;
     if (d.count < 0 || d.buf_depth < 0 || d.clamp_count < 0 || d.dup_target_count < 0 ||
-        (d.controller != NB2_ACT_PD && d.controller != NB2_ACT_PID)) {
+        d.controller < NB2_ACT_PD || d.controller > NB2_ACT_LSTM) {
         set_error("nb2_actuator_step: invalid count, buf_depth, clamp_count or controller");
         return NB2_ERR_INVALID_ARGUMENT;
     }
@@ -1076,10 +1076,29 @@ nb2_status nb2_actuator_step(const nb2_actuator_step_desc* desc, void* cuda_stre
         return NB2_ERR_INVALID_ARGUMENT;
     }
     if (d.count == 0) return NB2_OK;
+    const bool neural = d.controller == NB2_ACT_MLP || d.controller == NB2_ACT_LSTM;
     if (!d.indices || !d.pos_indices || !d.target_pos_indices || !d.effort_indices || !d.positions || !d.velocities || !d.target_pos ||
-        !d.target_vel || !d.kp || !d.kd || !d.output) {
+        !d.target_vel || (!neural && (!d.kp || !d.kd)) || !d.output) {
         set_error("nb2_actuator_step: NULL index, state, control, gain or output array");
         return NB2_ERR_INVALID_ARGUMENT;
+    }
+    if (neural) {
+        const nb2_actuator_network* w = d.network;
+        bool ok = w && w->weights && w->weight_count > 0 && w->layer_count >= 1 && w->layer_count <= NB2_NET_MAX_LAYERS &&
+                  w->state0_in && w->state1_in && w->state0_out && w->state1_out && w->state0_in != w->state0_out &&
+                  w->state1_in != w->state1_out;
+        if (ok && d.controller == NB2_ACT_MLP) {
+            ok = w->input_count >= 1 && w->input_count <= NB2_NET_MAX_INPUTS && w->widths[0] == 2 * w->input_count &&
+                 w->widths[w->layer_count] == 1 && w->history_length >= 1;
+            for (int l = 0; ok && l <= w->layer_count; ++l) ok = w->widths[l] >= 1;
+            for (int q = 0; ok && q < w->input_count; ++q) ok = w->input_idx[q] >= 0 && w->input_idx[q] < w->history_length;
+        } else if (ok) {
+            ok = w->widths[0] == 2 && w->widths[1] >= 1;
+        }
+        if (!ok) {
+            set_error("nb2_actuator_step: a network controller needs a valid nb2_actuator_network with weights and distinct state arrays");
+            return NB2_ERR_INVALID_ARGUMENT;
+        }
     }
     if (d.controller == NB2_ACT_PID && (!d.ki || !d.integral_max || !d.integral_in || !d.integral_out)) {
         set_error("nb2_actuator_step: PID needs ki, integral_max and the integral of both states");
@@ -1125,6 +1144,15 @@ nb2_status nb2_actuator_reset(int32_t count, int32_t buf_depth, const uint8_t* m
     }
     return launch_actuator_reset(count, buf_depth, mask, buf_pos, buf_vel, buf_act, num_pushes, write_idx, integral,
                                  static_cast<cudaStream_t>(cuda_stream));
+}
+
+nb2_status nb2_actuator_network_reset(int32_t count, int32_t rows, int32_t width, const uint8_t* mask, float* a, float* b,
+                                      void* cuda_stream) {
+    if (count < 0 || rows < 0 || width < 0) {
+        set_error("nb2_actuator_network_reset: invalid count, rows or width");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    return launch_actuator_network_reset(count, rows, width, mask, a, b, static_cast<cudaStream_t>(cuda_stream));
 }
 
 nb2_status nb2_actuator_param_gather(const int32_t* map, int32_t entries, const void* param, void* values, int32_t is_int,

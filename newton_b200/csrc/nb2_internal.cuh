@@ -261,6 +261,7 @@ nb2_status launch_actuator_step(const nb2_actuator_step_desc& desc, cudaStream_t
 nb2_status launch_joint_impedance_step(const nb2_joint_impedance_desc& desc, cudaStream_t s);
 nb2_status launch_actuator_reset(int count, int buf_depth, const uint8_t* mask, float* buf_pos, float* buf_vel, float* buf_act,
                                  int* num_pushes, int* write_idx, float* integral, cudaStream_t s);
+nb2_status launch_actuator_network_reset(int count, int rows, int width, const uint8_t* mask, float* a, float* b, cudaStream_t s);
 nb2_status launch_actuator_param(bool gather, const int* map, int entries, int dofs_per_world, const uint8_t* world_mask, const void* src,
                                  void* dst, bool is_int, cudaStream_t s);
 nb2_status launch_ik_solve(const nb2_ik_desc& desc, const float* joint_q_in, float* joint_q, float* joint_q_out, float* residuals, float* costs,

@@ -70,6 +70,10 @@ NB2_DEV float sin_w(float x) { return (float)sin((double)x); }
 NB2_DEV float cos_w(float x) { return (float)cos((double)x); }
 NB2_DEV float atan2_w(float y, float x) { return (float)atan2((double)y, (double)x); }
 NB2_DEV float log_w(float x) { return (float)log((double)x); }
+// activations of the learned actuator networks (include/newton_b200.h, the arithmetic contract of nb2_actuator_network)
+NB2_DEV float sigmoid_w(float a) { return (float)(1.0 / (1.0 + exp(-(double)a))); }
+NB2_DEV float tanh_w(float a) { return (float)tanh((double)a); }
+NB2_DEV float elu_w(float a, float alpha) { return a > 0.0f ? a : (float)((double)alpha * expm1((double)a)); }
 #else
 NB2_DEV float asin_w(float x) { return asinf(x); }
 NB2_DEV float acos_w(float x) { return acosf(x); }
@@ -77,7 +81,12 @@ NB2_DEV float sin_w(float x) { return sinf(x); }
 NB2_DEV float cos_w(float x) { return cosf(x); }
 NB2_DEV float atan2_w(float y, float x) { return atan2f(y, x); }
 NB2_DEV float log_w(float x) { return logf(x); }
+NB2_DEV float sigmoid_w(float a) { return 1.0f / (1.0f + expf(-a)); }
+NB2_DEV float tanh_w(float a) { return tanhf(a); }
+NB2_DEV float elu_w(float a, float alpha) { return a > 0.0f ? a : alpha * expm1f(a); }
 #endif
+NB2_DEV float softsign_w(float a) { return a / (1.0f + fabsf(a)); }
+NB2_DEV float relu_w(float a) { return a < 0.0f ? 0.0f : a; }  // torch.relu: NaN passes through
 
 struct Q4 {
     float x, y, z, w;

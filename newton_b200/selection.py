@@ -617,6 +617,16 @@ class ArticulationView:
         return out
 
     @staticmethod
+    def _actuator_param(component, name: str):
+        """``component.<name>``; the learned networks have no per-actuator parameters (their weights are shared by the group)."""
+        from .actuators.neural import NEURAL_CONTROLLERS
+
+        if isinstance(component, NEURAL_CONTROLLERS):
+            raise AttributeError(f"{type(component).__name__} has no per-actuator parameter '{name}': its network is shared by "
+                                 f"the whole group")
+        return getattr(component, name)
+
+    @staticmethod
     def _actuator_param_kind(param, name):
         if param.dtype == torch.float32:
             return 0
@@ -630,7 +640,7 @@ class ArticulationView:
         from .actuators.actuator import _call
 
         mapping = self._actuator_dof_mapping(actuator)
-        src = getattr(component, name)
+        src = self._actuator_param(component, name)
         is_int = self._actuator_param_kind(src, name)
         dst = torch.empty(mapping.numel(), dtype=src.dtype, device=self.device)
         if mapping.numel():
@@ -647,7 +657,7 @@ class ArticulationView:
 
         world_mask = self._resolve_world_mask(mask)
         mapping = self._actuator_dof_mapping(actuator)
-        dst = getattr(component, name)
+        dst = self._actuator_param(component, name)
         is_int = self._actuator_param_kind(dst, name)
         dpw = mapping.numel() // self.world_count if self.world_count else 0
         if not isinstance(values, torch.Tensor):
