@@ -4,14 +4,16 @@ Only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s ``cpu_baseline``
 legs may import this package.  The product path (``newton_b200``) never does and fails loudly without
 its CUDA library.
 
-``liboracle.so`` (built from ``oracle/oracle.cpp`` by ``oracle/Makefile``) restates the reference
+``liboracle.so`` (built by ``oracle/Makefile`` from every ``oracle/*.cpp``) restates the reference
 kernels of SURVEY.md §8(a) on the CPU; this module wraps it behind classes with the reference's own
-call signatures (``SolverXPBD.step``, ``CollisionPipeline.collide`` ...) operating on CPU tensors.
+call signatures (``SolverXPBD.step``, ``CollisionPipeline.collide`` ...) operating on CPU tensors.  The
+sub-modules (``oracle.dynamics``, ``oracle.actuator`` ...) wrap the other entry points of the same library.
 """
 
 from __future__ import annotations
 
 import ctypes as C
+import glob
 import os
 import subprocess
 
@@ -22,26 +24,29 @@ from newton_b200 import _abi
 from newton_b200.sim.model import Contacts
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
+_ROOT = os.path.dirname(_HERE)
+_SO = os.path.join(_HERE, "liboracle.so")
 _LIB = None
 
 
 def build(force: bool = False) -> str:
-    """Compile ``liboracle.so`` with g++ (``-ffp-contract=off``)."""
-    so = os.path.join(_HERE, "liboracle.so")
-    srcs = [os.path.join(_HERE, f) for f in os.listdir(_HERE) if f.endswith((".cpp", ".h"))]
-    srcs.append(os.path.join(_HERE, "..", "include", "newton_b200.h"))
-    if force or not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
-        subprocess.run(["make", "-C", _HERE, "-B" if force else "-s"], check=True, capture_output=True)
-    return so
+    """Run ``oracle/Makefile`` when ``liboracle.so`` is missing or older than a file it may compile; make then recompiles
+    the objects whose compiler-written dependency lists name a changed file.  Starts no process when the library is current."""
+    deps = [os.path.join(_HERE, "Makefile"), os.path.join(_ROOT, "include", "newton_b200.h")]
+    for pattern in ("oracle/*.cpp", "oracle/*.h", "newton_b200/csrc/*.cuh"):
+        deps += glob.glob(os.path.join(_ROOT, pattern))
+    if force or not os.path.exists(_SO) or any(os.path.getmtime(p) > os.path.getmtime(_SO) for p in deps):
+        subprocess.run(["make", "-C", _HERE, "-s", "-j", *(["-B"] if force else [])], check=True, capture_output=True)
+        os.utime(_SO)  # current now, even when the newer file was a header no object includes and make had nothing to do
+    return _SO
 
 
 def lib():
     global _LIB
     if _LIB is None:
-        so = os.path.join(_HERE, "liboracle.so")
-        if not os.path.exists(so):
+        if not os.path.exists(_SO):
             build()
-        _LIB = C.CDLL(so)
+        _LIB = C.CDLL(_SO)
         _LIB.orc_collide.restype = C.c_int
         _LIB.orc_collide_speculative.restype = C.c_int
         _LIB.orc_primitive_pair.restype = C.c_int

@@ -1,5 +1,4 @@
-// actuator.cpp - TEST INFRASTRUCTURE ONLY.  C export of oracle_actuator.h (liboracle_actuator.so, built by oracle/actuator.py
-// with the flags of oracle/Makefile), the CPU checker of newton_b200.actuators.
+// actuator.cpp - TEST INFRASTRUCTURE ONLY.  C export of oracle_actuator.h, the CPU checker of newton_b200.actuators.
 #include "oracle_actuator.h"
 
 extern "C" {

@@ -1,57 +1,51 @@
 """CPU oracle of the actuators - TEST INFRASTRUCTURE ONLY.
 
-``liboracle_actuator.so`` (``oracle/actuator.cpp`` + ``oracle_actuator.h``, compiled with the flags of ``oracle/Makefile``)
-restates the reference's actuator kernels serially, in thread-id order.  :func:`step`, :func:`reset` and :func:`host` run the
-product's own host code (``newton_b200.actuators``: descriptor construction, validation, duplicate tables, view mappings) on
-CPU tensors, with only the device launch replaced by the oracle's serial loops.
+``oracle/actuator.cpp`` + ``oracle_actuator.h`` restate the reference's actuator kernels serially, in thread-id order, and
+``oracle/neural_actuator.cpp`` + ``oracle_neural_actuator.h`` one step of a ``ControllerNeuralMLP`` / ``ControllerNeuralLSTM``
+group, under the arithmetic contract of ``include/newton_b200.h``.  :func:`step`, :func:`reset` and :func:`host` run the
+product's own host code (``newton_b200.actuators``: checkpoint loading, network extraction and packing, descriptor construction,
+validation, duplicate tables, view mappings) on CPU tensors, with only the device launch replaced by the oracle's serial loops.
 """
 
 from __future__ import annotations
 
 import contextlib
 import ctypes as C
-import os
-import subprocess
+import functools
 
-from .dynamics import _CXXFLAGS
+from newton_b200 import _abi
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SO = os.path.join(_HERE, "liboracle_actuator.so")
-_SOURCES = ("actuator.cpp", "oracle_actuator.h")
-_LIB = None
+from . import build, lib  # noqa: F401  (each module.build is oracle.build: they share one library)
 
 
-def build(force: bool = False) -> str:
-    """Compile ``liboracle_actuator.so`` with g++ (``-ffp-contract=off``: every fp32 operation rounds as written)."""
-    deps = [os.path.join(_HERE, f) for f in _SOURCES] + [os.path.join(_HERE, "..", "include", "newton_b200.h")]
-    if force or not os.path.exists(_SO) or any(os.path.getmtime(p) > os.path.getmtime(_SO) for p in deps):
-        cxx = os.environ.get("CXX", "g++")
-        subprocess.run([cxx, *_CXXFLAGS, "-shared", "-o", _SO, os.path.join(_HERE, "actuator.cpp")], check=True, capture_output=True)
-    return _SO
-
-
-def lib():
-    global _LIB
-    if _LIB is None:
-        if not os.path.exists(_SO):
-            build()
-        _LIB = C.CDLL(_SO)
-        P = C.c_void_p
-        _LIB.orc_actuator_step.argtypes = [P]
-        _LIB.orc_actuator_step.restype = None
-        _LIB.orc_actuator_reset.argtypes = [C.c_int32, C.c_int32, P, P, P, P, P, P, P]
-        _LIB.orc_actuator_reset.restype = None
-        _LIB.orc_actuator_param_copy.argtypes = [C.c_int32, P, C.c_int32, C.c_int32, P, P, P]
-        _LIB.orc_actuator_param_copy.restype = None
-    return _LIB
+@functools.cache
+def _lib():
+    L = lib()
+    P = C.c_void_p
+    L.orc_actuator_step.argtypes = [P]
+    L.orc_actuator_step.restype = None
+    L.orc_actuator_reset.argtypes = [C.c_int32, C.c_int32, P, P, P, P, P, P, P]
+    L.orc_actuator_reset.restype = None
+    L.orc_actuator_param_copy.argtypes = [C.c_int32, P, C.c_int32, C.c_int32, P, P, P]
+    L.orc_actuator_param_copy.restype = None
+    L.orc_neural_actuator_step.argtypes = [P]
+    L.orc_neural_actuator_step.restype = None
+    L.orc_neural_actuator_reset.argtypes = [C.c_int32, C.c_int32, C.c_int32, P, P, P]
+    L.orc_neural_actuator_reset.restype = None
+    return L
 
 
 def _backend(name, *args):
-    L = lib()
+    L = _lib()
     if name == "step":
-        L.orc_actuator_step(args[0])
+        if args[0]._obj.controller in (_abi.ACT_MLP, _abi.ACT_LSTM):
+            L.orc_neural_actuator_step(args[0])
+        else:
+            L.orc_actuator_step(args[0])
     elif name == "reset":
         L.orc_actuator_reset(*args)
+    elif name == "network_reset":
+        L.orc_neural_actuator_reset(*args)
     elif name == "param_gather":
         m, entries, src, dst, _is_int = args
         L.orc_actuator_param_copy(1, m, entries, 1, None, src, dst)
@@ -92,6 +86,7 @@ def step(actuator, sim_state, sim_control, current_act_state=None, next_act_stat
 
 
 def reset(state, mask=None) -> None:
-    """``<state>.reset(mask)`` on the CPU for an ``Actuator.State``, ``Delay.State`` or ``ControllerPID.State``."""
+    """``<state>.reset(mask)`` on the CPU for an ``Actuator.State``, ``Delay.State``, ``ControllerPID.State`` or a network
+    controller's state."""
     with host():
         state.reset(mask)

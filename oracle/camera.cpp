@@ -1,5 +1,4 @@
-// camera.cpp - TEST INFRASTRUCTURE ONLY.  C export of oracle_camera.h (liboracle_camera.so, built by oracle/camera.py with the
-// flags of oracle/Makefile), the CPU checker of newton_b200.sensors.SensorTiledCamera.
+// camera.cpp - TEST INFRASTRUCTURE ONLY.  C export of oracle_camera.h, the CPU checker of newton_b200.sensors.SensorTiledCamera.
 #include "oracle_camera.h"
 
 extern "C" {

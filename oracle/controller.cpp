@@ -1,5 +1,4 @@
-// controller.cpp - TEST INFRASTRUCTURE ONLY.  C export of oracle_controller.h (liboracle_controller.so, built by
-// oracle/controller.py with the flags of oracle/Makefile), the CPU checker of newton_b200.controllers.
+// controller.cpp - TEST INFRASTRUCTURE ONLY.  C export of oracle_controller.h, the CPU checker of newton_b200.controllers.
 #include "oracle_controller.h"
 
 extern "C" {

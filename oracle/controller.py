@@ -1,10 +1,9 @@
 """CPU oracle of the joint-impedance controllers - TEST INFRASTRUCTURE ONLY.
 
-``liboracle_controller.so`` (``oracle/controller.cpp`` + ``oracle_controller.h``, compiled with the flags of ``oracle/Makefile``)
-restates the reference's model-free step serially.  :func:`step` runs the product's own host code
-(``newton_b200.controllers``: validation, index normalisation, the descriptor) on CPU tensors, with only the device launch
-replaced.  For ``ControllerJointImpedance`` the replacement composes the reference's model-based step from the oracle's own
-pieces: the gather into the internal state, :func:`oracle.eval_fk`, :func:`oracle.dynamics.eval_mass_matrix`,
+``oracle/controller.cpp`` + ``oracle_controller.h`` restate the reference's model-free step serially.  :func:`step` runs the
+product's own host code (``newton_b200.controllers``: validation, index normalisation, the descriptor) on CPU tensors, with only
+the device launch replaced.  For ``ControllerJointImpedance`` the replacement composes the reference's model-based step from the
+oracle's own pieces: the gather into the internal state, :func:`oracle.eval_fk`, :func:`oracle.dynamics.eval_mass_matrix`,
 :func:`oracle.dynamics.eval_inverse_dynamics_passive` and the model-free law on their outputs.
 """
 
@@ -12,38 +11,20 @@ from __future__ import annotations
 
 import contextlib
 import ctypes as C
-import os
-import subprocess
+import functools
 
-from .dynamics import _CXXFLAGS
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SO = os.path.join(_HERE, "liboracle_controller.so")
-_SOURCES = ("controller.cpp", "oracle_controller.h")
-_LIB = None
+from . import build, lib  # noqa: F401  (each module.build is oracle.build: they share one library)
 
 
-def build(force: bool = False) -> str:
-    """Compile ``liboracle_controller.so`` with g++ (``-ffp-contract=off``: every fp32 operation rounds as written)."""
-    deps = [os.path.join(_HERE, f) for f in _SOURCES] + [os.path.join(_HERE, "..", "include", "newton_b200.h")]
-    if force or not os.path.exists(_SO) or any(os.path.getmtime(p) > os.path.getmtime(_SO) for p in deps):
-        cxx = os.environ.get("CXX", "g++")
-        subprocess.run([cxx, *_CXXFLAGS, "-shared", "-o", _SO, os.path.join(_HERE, "controller.cpp")], check=True, capture_output=True)
-    return _SO
+@functools.cache
+def _lib():
+    from newton_b200 import _abi
 
-
-def lib():
-    global _LIB
-    if _LIB is None:
-        if not os.path.exists(_SO):
-            build()
-        from newton_b200 import _abi
-
-        _LIB = C.CDLL(_SO)
-        for name in ("orc_joint_impedance_gather_state", "orc_joint_impedance_step"):
-            getattr(_LIB, name).argtypes = [C.POINTER(_abi.JointImpedanceDesc)]
-            getattr(_LIB, name).restype = None
-    return _LIB
+    L = lib()
+    for name in ("orc_joint_impedance_gather_state", "orc_joint_impedance_step"):
+        getattr(L, name).argtypes = [C.POINTER(_abi.JointImpedanceDesc)]
+        getattr(L, name).restype = None
+    return L
 
 
 def _model_based(controller, desc) -> None:
@@ -53,7 +34,7 @@ def _model_based(controller, desc) -> None:
     import oracle.dynamics as dyn
     from newton_b200 import _abi
 
-    L = lib()
+    L = _lib()
     L.orc_joint_impedance_gather_state(C.byref(desc))
     model, state = controller._model, controller._state
     use_g, use_c, use_m = bool(desc.use_gravity), bool(desc.use_coriolis), bool(desc.use_inertia)
@@ -88,7 +69,7 @@ def host():
         elif controller._model is not None:
             _model_based(controller, desc)
         else:
-            lib().orc_joint_impedance_step(C.byref(desc))
+            _lib().orc_joint_impedance_step(C.byref(desc))
 
     J._launch = launch
     try:

@@ -1,5 +1,5 @@
-// dynamics.cpp - TEST INFRASTRUCTURE ONLY.  C exports of oracle_dynamics.h (liboracle_dynamics.so, built by oracle/dynamics.py with
-// the flags of oracle/Makefile), the CPU checker of newton_b200.eval_jacobian / eval_mass_matrix / eval_inverse_dynamics_*.
+// dynamics.cpp - TEST INFRASTRUCTURE ONLY.  C exports of oracle_dynamics.h, the CPU checker of newton_b200.eval_jacobian /
+// eval_mass_matrix / eval_inverse_dynamics_*.
 #include "oracle_dynamics.h"
 
 using namespace orc;

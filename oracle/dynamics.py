@@ -1,45 +1,20 @@
 """CPU oracle of the articulation dynamics queries - TEST INFRASTRUCTURE ONLY.
 
-``liboracle_dynamics.so`` (``oracle/dynamics.cpp`` + ``oracle_dynamics.h``, compiled with the flags of ``oracle/Makefile``)
-restates the reference's ``newton.eval_jacobian`` / ``eval_mass_matrix`` / ``eval_inverse_dynamics_passive`` /
-``eval_inverse_dynamics_force`` serially, one function per reference function.  The wrappers take the reference's call
-signatures and work on CPU models and tensors; outputs are float32 tensors.
+``oracle/dynamics.cpp`` + ``oracle_dynamics.h`` restate the reference's ``newton.eval_jacobian`` / ``eval_mass_matrix`` /
+``eval_inverse_dynamics_passive`` / ``eval_inverse_dynamics_force`` serially, one function per reference function.  The wrappers
+take the reference's call signatures and work on CPU models and tensors; outputs are float32 tensors.
 """
 
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import torch
 
 from newton_b200 import _abi
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SO = os.path.join(_HERE, "liboracle_dynamics.so")
-_SOURCES = ("dynamics.cpp", "oracle_dynamics.h", "oracle_featherstone.h", "oracle_xpbd.h", "oracle_math.h")
-_LIB = None
-_CXXFLAGS = ["-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-Wall", "-Wno-unused-function", "-Wno-unknown-pragmas"]
-
-
-def build(force: bool = False) -> str:
-    """Compile ``liboracle_dynamics.so`` with g++ (``-ffp-contract=off``: every fp32 operation rounds as written)."""
-    deps = [os.path.join(_HERE, f) for f in _SOURCES] + [os.path.join(_HERE, "..", "include", "newton_b200.h")]
-    if force or not os.path.exists(_SO) or any(os.path.getmtime(p) > os.path.getmtime(_SO) for p in deps):
-        cxx = os.environ.get("CXX", "g++")
-        subprocess.run([cxx, *_CXXFLAGS, "-shared", "-o", _SO, os.path.join(_HERE, "dynamics.cpp")], check=True, capture_output=True)
-    return _SO
-
-
-def lib():
-    global _LIB
-    if _LIB is None:
-        if not os.path.exists(_SO):
-            build()
-        _LIB = C.CDLL(_SO)
-    return _LIB
+from . import build, lib  # noqa: F401  (each module.build is oracle.build: they share one library)
 
 
 def _check_cpu(model):

@@ -1,6 +1,5 @@
-// ik.cpp - TEST INFRASTRUCTURE ONLY.  C exports of oracle_ik.h (liboracle_ik.so, built by oracle/ik.py with the flags of
-// oracle/Makefile), the CPU checker of newton_b200.ik.  The entries take the arguments of nb2_ik_solve / nb2_ik_sample /
-// nb2_ik_select without the stream, on host arrays.
+// ik.cpp - TEST INFRASTRUCTURE ONLY.  C exports of oracle_ik.h, the CPU checker of newton_b200.ik.  The entries take the
+// arguments of nb2_ik_solve / nb2_ik_sample / nb2_ik_select without the stream, on host arrays.
 #include <cstring>
 
 #include "oracle_ik.h"

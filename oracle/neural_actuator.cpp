@@ -1,5 +1,5 @@
-// neural_actuator.cpp - TEST INFRASTRUCTURE ONLY.  C export of oracle_neural_actuator.h (liboracle_neural_actuator.so, built by
-// oracle/neural_actuator.py with the flags of oracle/Makefile), the CPU checker of the learned actuator networks.
+// neural_actuator.cpp - TEST INFRASTRUCTURE ONLY.  C export of oracle_neural_actuator.h, the CPU checker of the learned
+// actuator networks.
 #include "oracle_neural_actuator.h"
 
 extern "C" {

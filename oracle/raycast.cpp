@@ -1,5 +1,5 @@
-// raycast.cpp - TEST INFRASTRUCTURE ONLY.  C export of oracle_raycast.h (liboracle_raycast.so, built by oracle/raycast.py with the
-// flags of oracle/Makefile), the CPU checker of newton_b200.intersect_ray and Model.bvh_refit_shapes.
+// raycast.cpp - TEST INFRASTRUCTURE ONLY.  C export of oracle_raycast.h, the CPU checker of newton_b200.intersect_ray and
+// Model.bvh_refit_shapes.
 #include "oracle_raycast.h"
 
 extern "C" {

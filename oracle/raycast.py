@@ -1,18 +1,16 @@
 """CPU oracle of ray casting - TEST INFRASTRUCTURE ONLY.
 
-``liboracle_raycast.so`` (``oracle/raycast.cpp`` + ``oracle_raycast.h``, compiled with the flags of ``oracle/Makefile``)
-restates the reference's shape transforms and bounds kernels, its per-primitive ray tests and ``intersect_ray`` as an
-exhaustive loop: every enabled shape of the ray's group behind an AABB pre-test, and every triangle of a mesh, with no BVH.
-:func:`refit_shapes` and :func:`intersect_ray` take the product's signatures and work on CPU models: the group layout is the
-product's host table (``Model.bvh_build_shapes``), the triangles are the oracle's own, in face order, taken from each
-shape's ``Mesh``.
+``oracle/raycast.cpp`` + ``oracle_raycast.h`` restate the reference's shape transforms and bounds kernels, its per-primitive
+ray tests and ``intersect_ray`` as an exhaustive loop: every enabled shape of the ray's group behind an AABB pre-test, and every
+triangle of a mesh, with no BVH.  :func:`refit_shapes` and :func:`intersect_ray` take the product's signatures and work on CPU
+models: the group layout is the product's host table (``Model.bvh_build_shapes``), the triangles are the oracle's own, in face
+order, taken from each shape's ``Mesh``.
 """
 
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
+import functools
 
 import numpy as np
 
@@ -20,35 +18,18 @@ from newton_b200 import _abi
 from newton_b200.geometry import raycast as _product
 from newton_b200.sim.enums import GeoType
 
-from .dynamics import _CXXFLAGS
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SO = os.path.join(_HERE, "liboracle_raycast.so")
-_SOURCES = ("raycast.cpp", "oracle_raycast.h", "oracle_math.h")
-_LIB = None
+from . import build, lib  # noqa: F401  (each module.build is oracle.build: they share one library)
 
 
-def build(force: bool = False) -> str:
-    """Compile ``liboracle_raycast.so`` with g++ (``-ffp-contract=off``: every fp32 operation rounds as written)."""
-    deps = [os.path.join(_HERE, f) for f in _SOURCES] + [os.path.join(_HERE, "..", "include", "newton_b200.h")]
-    if force or not os.path.exists(_SO) or any(os.path.getmtime(p) > os.path.getmtime(_SO) for p in deps):
-        cxx = os.environ.get("CXX", "g++")
-        subprocess.run([cxx, *_CXXFLAGS, "-shared", "-o", _SO, os.path.join(_HERE, "raycast.cpp")], check=True, capture_output=True)
-    return _SO
-
-
-def lib():
-    global _LIB
-    if _LIB is None:
-        if not os.path.exists(_SO):
-            build()
-        _LIB = C.CDLL(_SO)
-        P = C.c_void_p
-        _LIB.orc_raycast_refit.argtypes = [C.POINTER(_abi.RaycastView), P]
-        _LIB.orc_raycast_refit.restype = None
-        _LIB.orc_intersect_ray.argtypes = [C.POINTER(_abi.RaycastView), P, P, P, C.c_int, P, P, P, C.c_int, P, P, P]
-        _LIB.orc_intersect_ray.restype = None
-    return _LIB
+@functools.cache
+def _lib():
+    L = lib()
+    P = C.c_void_p
+    L.orc_raycast_refit.argtypes = [C.POINTER(_abi.RaycastView), P]
+    L.orc_raycast_refit.restype = None
+    L.orc_intersect_ray.argtypes = [C.POINTER(_abi.RaycastView), P, P, P, C.c_int, P, P, P, C.c_int, P, P, P]
+    L.orc_intersect_ray.restype = None
+    return L
 
 
 def _require_cpu(model):
@@ -83,7 +64,7 @@ def refit_shapes(model, state) -> None:
     if getattr(model, "bvh_shape_enabled", None) is None:
         raise RuntimeError(_product._REFIT_BEFORE_BUILD)
     bq = _abi.ptr(getattr(state, "body_q", None), "f32", "cpu", 7 * int(model.body_count), "state.body_q")
-    lib().orc_raycast_refit(C.byref(_product.raycast_view(model)), C.c_void_p(bq))
+    _lib().orc_raycast_refit(C.byref(_product.raycast_view(model)), C.c_void_p(bq))
 
 
 def intersect_ray(model, *, ray_origins, ray_directions, ray_worlds, enable_global_world: bool = True, out_dist=None,
@@ -100,5 +81,5 @@ def intersect_ray(model, *, ray_origins, ray_directions, ray_worlds, enable_glob
     od = _abi.ptr(out_dist, "f32", "cpu", n, "out_dist")
     oi = _abi.ptr(out_shape_id, "i32", "cpu", n, "out_shape_id")
     on = _abi.ptr(out_normal, "f32", "cpu", 3 * n, "out_normal")
-    lib().orc_intersect_ray(C.byref(_product.raycast_view(model)), start.ctypes.data, count.ctypes.data,
-                            tris.ctypes.data if tris.size else None, n, o, d, w, 1 if enable_global_world else 0, od, oi, on)
+    _lib().orc_intersect_ray(C.byref(_product.raycast_view(model)), start.ctypes.data, count.ctypes.data,
+                             tris.ctypes.data if tris.size else None, n, o, d, w, 1 if enable_global_world else 0, od, oi, on)

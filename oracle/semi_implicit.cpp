@@ -1,5 +1,5 @@
-// semi_implicit.cpp - TEST INFRASTRUCTURE ONLY.  C export of oracle_semi_implicit.h (liboracle_semi_implicit.so, built by
-// oracle/semi_implicit.py with the flags of oracle/Makefile), the CPU checker of newton_b200.solvers.SolverSemiImplicit.
+// semi_implicit.cpp - TEST INFRASTRUCTURE ONLY.  C export of oracle_semi_implicit.h, the CPU checker of
+// newton_b200.solvers.SolverSemiImplicit.
 #include "oracle_semi_implicit.h"
 
 extern "C" {

@@ -1,5 +1,4 @@
-// sensor.cpp - TEST INFRASTRUCTURE ONLY.  C export of oracle_sensor.h (liboracle_sensor.so, built by oracle/sensor.py with the
-// flags of oracle/Makefile), the CPU checker of newton_b200.sensors.SensorContact.
+// sensor.cpp - TEST INFRASTRUCTURE ONLY.  C export of oracle_sensor.h, the CPU checker of newton_b200.sensors.SensorContact.
 #include "oracle_sensor.h"
 
 extern "C" {

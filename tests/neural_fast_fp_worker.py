@@ -14,7 +14,7 @@ sys.path.insert(0, ROOT)
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
-import oracle.neural_actuator as on  # noqa: E402
+import oracle.actuator as on  # noqa: E402
 from newton_b200 import _lib  # noqa: E402
 from newton_b200.actuators import Actuator, ControllerNeuralLSTM, ControllerNeuralMLP  # noqa: E402
 from tests import neural_nets as NN  # noqa: E402

@@ -25,9 +25,10 @@ from newton_b200.actuators import (
 
 @pytest.fixture(scope="module")
 def oact():
+    import oracle
     import oracle.actuator as oact
 
-    oact.build()
+    oracle.build()
     return oact
 
 

@@ -162,7 +162,6 @@ def fk_state(oracle, model, joint_qd=None):
 def od(oracle_lib):
     import oracle.dynamics as od
 
-    od.build()
     return od
 
 

@@ -35,9 +35,10 @@ STATE_ARRAYS = (("controller_state", "integral"), ("delay_state", "buffer_pos"),
 
 @pytest.fixture(scope="module")
 def oact():
+    import oracle
     import oracle.actuator as oact
 
-    oact.build()
+    oracle.build()
     return oact
 
 

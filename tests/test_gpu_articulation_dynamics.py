@@ -18,7 +18,6 @@ pytestmark = pytest.mark.gpu
 def od(oracle_lib):
     import oracle.dynamics as od
 
-    od.build()
     return od
 
 

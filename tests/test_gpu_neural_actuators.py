@@ -33,9 +33,10 @@ DEV = "cuda:0"
 
 @pytest.fixture(scope="module")
 def on():
-    import oracle.neural_actuator as on
+    import oracle
+    import oracle.actuator as on
 
-    on.build()
+    oracle.build()
     return on
 
 

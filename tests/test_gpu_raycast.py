@@ -21,9 +21,10 @@ DEV = "cuda:0"
 
 @pytest.fixture(scope="module")
 def oray():
+    import oracle
     import oracle.raycast as oray
 
-    oray.build()
+    oracle.build()
     return oray
 
 

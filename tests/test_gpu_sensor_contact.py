@@ -23,9 +23,10 @@ DEV = "cuda:0"
 
 @pytest.fixture(scope="module")
 def osensor():
+    import oracle
     import oracle.sensor as osensor
 
-    osensor.build()
+    oracle.build()
     return osensor
 
 

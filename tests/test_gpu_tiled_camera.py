@@ -29,11 +29,10 @@ SUBSETS = [("depth",), ("forward_depth",), ("shape_index",), ("normal",), ("dept
 
 @pytest.fixture(scope="module")
 def ocam():
+    import oracle
     import oracle.camera as ocam
-    import oracle.raycast
 
-    oracle.raycast.build()
-    ocam.build()
+    oracle.build()
     return ocam
 
 

@@ -30,9 +30,10 @@ from tests import test_actuators as T
 
 @pytest.fixture(scope="module")
 def on():
-    import oracle.neural_actuator as on
+    import oracle
+    import oracle.actuator as on
 
-    on.build()
+    oracle.build()
     return on
 
 

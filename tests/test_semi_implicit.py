@@ -23,9 +23,10 @@ from tests import semi_implicit_cases as cases
 
 @pytest.fixture(scope="module")
 def si():
+    import oracle
     import oracle.semi_implicit
 
-    oracle.semi_implicit.build()
+    oracle.build()
     return oracle.semi_implicit
 
 

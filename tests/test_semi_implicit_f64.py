@@ -34,7 +34,6 @@ NEAR_CONTACTS = 1.0e-4
 def oracle_si(oracle_lib):
     import oracle.semi_implicit
 
-    oracle.semi_implicit.build()
     return oracle.semi_implicit.SolverSemiImplicit
 
 

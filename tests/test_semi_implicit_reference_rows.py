@@ -22,7 +22,6 @@ def si():
     import oracle.semi_implicit
 
     oracle.build()
-    oracle.semi_implicit.build()
     return oracle.semi_implicit
 
 

@@ -15,9 +15,10 @@ from newton_b200.utils import xform as X
 
 @pytest.fixture(scope="module")
 def osensor():
+    import oracle
     import oracle.sensor as osensor
 
-    osensor.build()
+    oracle.build()
     return osensor
 
 

@@ -27,11 +27,10 @@ LOOK_UP = (1.0, 0.0, 0.0, 0.0)  # 180 deg about x: the camera looks up +z
 
 @pytest.fixture(scope="module")
 def ocam():
+    import oracle
     import oracle.camera as ocam
-    import oracle.raycast
 
-    oracle.raycast.build()
-    ocam.build()
+    oracle.build()
     return ocam
 
 
