@@ -462,6 +462,49 @@ nb2_status nb2_sensor_contact_scratch_bytes(int32_t rigid_contact_max, int32_t r
 nb2_status nb2_sensor_contact_update(const nb2_sensor_contact_view* sensor, const nb2_contacts_view* contacts, const float* body_q,
                                      void* scratch, size_t scratch_bytes, void* cuda_stream);
 
+/* --- site sensors (reference newton.sensors.SensorFrameTransform / SensorIMU, sensors/sensor_frame_transform.py, sensor_imu.py)
+ * A site is a shape flagged ShapeFlags.SITE, with no mass and no contacts; the sensors read it through the ordinary shape arrays.  The
+ * index tables are built once by the caller (newton_b200.sensors, on the host) and trusted: every id must lie in range.  The world
+ * transform of shape s is X_w(s) = shape_body[s] >= 0 ? body_q[shape_body[s]] * shape_transform[s] : shape_transform[s] (a static
+ * shape's transform is copied, not multiplied by the identity).  Each update is one launch, one thread per output; nothing is
+ * allocated or synchronised, so an update can be captured into a CUDA graph.  count == 0 launches nothing. */
+typedef struct nb2_sensor_frame_transform_view {
+    int32_t count;                  /* outputs */
+    int32_t body_count;             /* rows of body_q; body_q may be NULL when 0 */
+    const int32_t* shapes;          /* [count] shape whose pose is measured */
+    const int32_t* references;      /* [count] reference site of each output (a single reference already repeated) */
+    const int32_t* shape_body;      /* Model.shape_body */
+    const float* shape_transform;   /* Model.shape_transform */
+    float* transforms;              /* [count, 7] output: inverse(X_w(reference)) * X_w(shape) */
+} nb2_sensor_frame_transform_view;
+
+/* Reference SensorFrameTransform.update: compute_shape_transforms_kernel and compute_relative_transforms_kernel fused.  The
+ * reference's intermediate per-shape buffer is float32 as well, so fusing changes no bit. */
+nb2_status nb2_sensor_frame_transform_update(const nb2_sensor_frame_transform_view* sensor, const float* body_q, void* cuda_stream);
+
+typedef struct nb2_sensor_imu_view {
+    int32_t count;                  /* sensors */
+    int32_t body_count;             /* rows of body_q / body_qd / body_qdd; they may be NULL when 0 */
+    int32_t gravity_count;          /* rows of gravity: world w reads gravity[w], world -1 reads gravity[gravity_count - 1] */
+    const int32_t* sites;           /* [count] site of each sensor */
+    const int32_t* shape_body;      /* Model.shape_body */
+    const int32_t* shape_world;     /* Model.shape_world */
+    const float* shape_transform;   /* Model.shape_transform */
+    const int32_t* body_world;      /* Model.body_world */
+    const float* body_com;          /* Model.body_com */
+    const float* gravity;           /* Model.gravity, vec3[gravity_count] */
+    float* accelerometer;           /* [count, 3] output, site frame */
+    float* gyroscope;               /* [count, 3] output, site frame */
+} nb2_sensor_imu_view;
+
+/* Reference SensorIMU.update (compute_sensor_imu_kernel), in its operation order.  For a site on body b with X_bs = (p, q_s):
+ *   r = quat_rotate(q_b, p - body_com[b]);  a = ((top(qdd_b) - g) + cross(bottom(qdd_b), r)) + cross(w_b, cross(w_b, r))
+ *   accelerometer = quat_rotate_inv(q_b * q_s, a);  gyroscope = quat_rotate_inv(q_b * q_s, w_b)   (w_b = bottom(body_qd[b]))
+ * with g the gravity of body_world[b].  A body-less site reads quat_rotate_inv(q_s, -g) with the gravity of shape_world[s] and a
+ * zero gyroscope. */
+nb2_status nb2_sensor_imu_update(const nb2_sensor_imu_view* sensor, const float* body_q, const float* body_qd, const float* body_qdd,
+                                 void* cuda_stream);
+
 /* --- ray casting (reference newton.intersect_ray, geometry/raycast.py; Model.bvh_build_shapes / bvh_refit_shapes) ----------
  * The host (newton_b200.geometry.raycast) groups the enabled shapes by world: group w in [0, W) holds world w's shapes, group W
  * the global (world -1) shapes, each in ascending shape id; enabled[group_start[g] .. group_start[g + 1]) are group g's shape ids.

@@ -223,6 +223,21 @@ class SensorContactView(C.Structure):
 SENSING_SHAPE, SENSING_BODY = 1, 2  # NB2_SENSING_* (the reference's _SENSING_KIND_* values)
 
 
+class SensorFrameTransformView(C.Structure):
+    """``nb2_sensor_frame_transform_view``"""
+
+    _fields_ = [("count", C.c_int32), ("body_count", C.c_int32), ("shapes", C.c_void_p), ("references", C.c_void_p),
+                ("shape_body", C.c_void_p), ("shape_transform", C.c_void_p), ("transforms", C.c_void_p)]
+
+
+class SensorIMUView(C.Structure):
+    """``nb2_sensor_imu_view``"""
+
+    _fields_ = [("count", C.c_int32), ("body_count", C.c_int32), ("gravity_count", C.c_int32), ("sites", C.c_void_p),
+                ("shape_body", C.c_void_p), ("shape_world", C.c_void_p), ("shape_transform", C.c_void_p), ("body_world", C.c_void_p),
+                ("body_com", C.c_void_p), ("gravity", C.c_void_p), ("accelerometer", C.c_void_p), ("gyroscope", C.c_void_p)]
+
+
 class RaycastView(C.Structure):
     """``nb2_raycast_view``"""
 
@@ -410,7 +425,7 @@ def state_view(state, model=None) -> StateView:
     dev = getattr(model, "device", None)
     nb = int(getattr(model, "body_count", 0)) if model is not None else None
     need = {} if model is None else {
-        "body_q": 7 * nb, "body_qd": 6 * nb, "body_f": 6 * nb, "body_parent_f": 6 * nb,
+        "body_q": 7 * nb, "body_qd": 6 * nb, "body_f": 6 * nb, "body_parent_f": 6 * nb, "body_qdd": 6 * nb,
         "joint_q": int(model.joint_coord_count), "joint_qd": int(model.joint_dof_count)}
     for name, _ in StateView._fields_:
         setattr(v, name, ptr(getattr(state, name, None), "f32", dev, need.get(name), "state." + name))

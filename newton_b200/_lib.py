@@ -28,7 +28,7 @@ EXPORTED_SYMBOLS = (
     "nb2_model_create", "nb2_model_destroy", "nb2_model_notify_changed", "nb2_model_rigid_contact_max", "nb2_collide_configure", "nb2_collide", "nb2_collide_speculative", "nb2_contacts_match", "nb2_contacts_sort", "nb2_contacts_import",
     "nb2_xpbd_step", "nb2_xpbd_update_contacts", "nb2_integrate_bodies", "nb2_featherstone_step", "nb2_semi_implicit_step", "nb2_eval_fk", "nb2_eval_ik", "nb2_eval_fk_masked",
     "nb2_eval_jacobian", "nb2_eval_mass_matrix", "nb2_eval_inverse_dynamics_passive", "nb2_eval_inverse_dynamics_force",
-    "nb2_sensor_contact_scratch_bytes", "nb2_sensor_contact_update", "nb2_raycast_refit", "nb2_intersect_ray",
+    "nb2_sensor_contact_scratch_bytes", "nb2_sensor_contact_update", "nb2_sensor_frame_transform_update", "nb2_sensor_imu_update", "nb2_raycast_refit", "nb2_intersect_ray",
     "nb2_camera_render", "nb2_actuator_step", "nb2_actuator_reset", "nb2_actuator_network_reset", "nb2_actuator_param_gather", "nb2_actuator_param_scatter",
     "nb2_joint_impedance_step",
     "nb2_ik_solve", "nb2_ik_sample", "nb2_ik_select",
@@ -104,6 +104,10 @@ def lib():
         L.nb2_sensor_contact_scratch_bytes.restype = C.c_int
         L.nb2_sensor_contact_update.argtypes = [C.POINTER(_abi.SensorContactView), C.POINTER(_abi.ContactsView), P, P, C.c_size_t, P]
         L.nb2_sensor_contact_update.restype = C.c_int
+        L.nb2_sensor_frame_transform_update.argtypes = [C.POINTER(_abi.SensorFrameTransformView), P, P]
+        L.nb2_sensor_frame_transform_update.restype = C.c_int
+        L.nb2_sensor_imu_update.argtypes = [C.POINTER(_abi.SensorIMUView), P, P, P, P]
+        L.nb2_sensor_imu_update.restype = C.c_int
         L.nb2_raycast_refit.argtypes = [C.POINTER(_abi.RaycastView), P, P]
         L.nb2_raycast_refit.restype = C.c_int
         L.nb2_intersect_ray.argtypes = [C.POINTER(_abi.RaycastView), C.c_int32, P, P, P, C.c_int32, P, P, P, P]

@@ -905,6 +905,41 @@ nb2_status nb2_sensor_contact_update(const nb2_sensor_contact_view* sensor, cons
     return launch_sensor_contact_update(s, c, body_q, scratch, scratch_bytes, static_cast<cudaStream_t>(cuda_stream));
 }
 
+nb2_status nb2_sensor_frame_transform_update(const nb2_sensor_frame_transform_view* sensor, const float* body_q, void* cuda_stream) {
+    if (!sensor || sensor->count < 0 || sensor->body_count < 0) {
+        set_error("nb2_sensor_frame_transform_update: NULL sensor or negative count");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    const nb2_sensor_frame_transform_view& s = *sensor;
+    if (s.count > 0 && (!s.shapes || !s.references || !s.shape_body || !s.shape_transform || !s.transforms || (s.body_count > 0 && !body_q))) {
+        set_error("nb2_sensor_frame_transform_update: NULL array (shapes, references, shape_body, shape_transform, transforms or body_q)");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    return launch_sensor_frame_transform_update(s, body_q, static_cast<cudaStream_t>(cuda_stream));
+}
+
+nb2_status nb2_sensor_imu_update(const nb2_sensor_imu_view* sensor, const float* body_q, const float* body_qd, const float* body_qdd,
+                                 void* cuda_stream) {
+    if (!sensor || sensor->count < 0 || sensor->body_count < 0 || sensor->gravity_count < 0) {
+        set_error("nb2_sensor_imu_update: NULL sensor or negative count");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    const nb2_sensor_imu_view& s = *sensor;
+    if (s.count > 0 && (!s.sites || !s.shape_body || !s.shape_world || !s.shape_transform || !s.accelerometer || !s.gyroscope)) {
+        set_error("nb2_sensor_imu_update: NULL array (sites, shape_body, shape_world, shape_transform, accelerometer or gyroscope)");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    if (s.count > 0 && (s.gravity_count < 1 || !s.gravity)) {
+        set_error("nb2_sensor_imu_update: gravity needs at least one entry");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    if (s.count > 0 && s.body_count > 0 && (!s.body_world || !s.body_com || !body_q || !body_qd || !body_qdd)) {
+        set_error("nb2_sensor_imu_update: NULL body array (body_world, body_com, body_q, body_qd or body_qdd)");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    return launch_sensor_imu_update(s, body_q, body_qd, body_qdd, static_cast<cudaStream_t>(cuda_stream));
+}
+
 static bool raycast_view_valid(const nb2_raycast_view* v, const char* what) {
     if (!v) {
         set_error(std::string(what) + ": NULL view");

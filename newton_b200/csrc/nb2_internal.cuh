@@ -253,6 +253,9 @@ nb2_status launch_eval_inverse_dynamics_force(nb2_model* m, const float* body_q,
 nb2_status sensor_contact_scratch_bytes(int rigid_contact_max, int row_count, int col_count, size_t* bytes);
 nb2_status launch_sensor_contact_update(const nb2_sensor_contact_view& sensor, const nb2_contacts_view& contacts, const float* body_q,
                                         void* scratch, size_t scratch_bytes, cudaStream_t s);
+nb2_status launch_sensor_frame_transform_update(const nb2_sensor_frame_transform_view& sensor, const float* body_q, cudaStream_t s);
+nb2_status launch_sensor_imu_update(const nb2_sensor_imu_view& sensor, const float* body_q, const float* body_qd, const float* body_qdd,
+                                    cudaStream_t s);
 nb2_status launch_raycast_refit(const nb2_raycast_view& v, const float* body_q, cudaStream_t s);
 nb2_status launch_intersect_ray(const nb2_raycast_view& v, int ray_count, const float* origins, const float* directions, const int* worlds,
                                 bool enable_global_world, float* out_dist, int* out_shape_id, float* out_normal, cudaStream_t s);

@@ -14,6 +14,10 @@
 //      written whole.  A second walk over the run divides each touched position entry by its weight, once, and the thread
 //      finally writes the sensing transform.
 // The caller owns all memory (outputs and one scratch buffer); nothing here allocates or synchronises.
+//
+// Site sensors (reference SensorFrameTransform, SensorIMU): one launch each, one thread per output, straight from the model's
+// shape arrays and the state.  Both share shape_world_xform with the contact sensor's sensing transforms: the reference copies a
+// static shape's transform rather than multiplying it by the identity, which could turn a -0 component into +0.
 #include <cub/device/device_radix_sort.cuh>
 
 #include "nb2_internal.cuh"
@@ -117,6 +121,14 @@ __global__ void __launch_bounds__(256) sensor_records_kernel(nb2_sensor_contact_
 
 NB2_DEV void add3(float* p, V3 v) { st3(p, ld3(p) + v); }
 
+// World transform of shape s: body_q[b] * shape_transform[s] on a body, shape_transform[s] for a static shape.
+NB2_DEV Xf shape_world_xform(const float* __restrict__ body_q, const int* __restrict__ shape_body, const float* __restrict__ shape_transform,
+                             int s) {
+    const int b = shape_body[s];
+    const Xf Xs = ldx(shape_transform + 7 * size_t(s));
+    return b >= 0 ? xmul(ldx(body_q + 7 * size_t(b)), Xs) : Xs;
+}
+
 // The atomics of accumulate_contact_forces_kernel in serial order, normalize_contact_positions_kernel (:159-168) and
 // compute_sensing_transforms_kernel (:44-64) for one row.
 __global__ void __launch_bounds__(128) sensor_rows_kernel(nb2_sensor_contact_view S, const float* __restrict__ body_q, int N,
@@ -176,18 +188,65 @@ __global__ void __launch_bounds__(128) sensor_rows_kernel(nb2_sensor_contact_vie
         }
     }
     const int idx = S.sensing_indices[r];
-    Xf X;
-    if (S.sensing_kind == NB2_SENSING_BODY) {
-        X = ldx(body_q + 7 * size_t(idx));
-    } else {
-        const int b = S.shape_body[idx];
-        const Xf Xs = ldx(S.shape_transform + 7 * size_t(idx));
-        X = b >= 0 ? xmul(ldx(body_q + 7 * size_t(b)), Xs) : Xs;
-    }
+    const Xf X = S.sensing_kind == NB2_SENSING_BODY ? ldx(body_q + 7 * size_t(idx)) : shape_world_xform(body_q, S.shape_body, S.shape_transform, idx);
     stx(S.sensing_transforms + 7 * size_t(r), X);
 }
 
+// compute_shape_transforms_kernel + compute_relative_transforms_kernel (sensor_frame_transform.py:16-78): X_ro = inverse(X_wr) * X_wo.
+__global__ void __launch_bounds__(128) sensor_frame_transform_kernel(const nb2_sensor_frame_transform_view S, const float* __restrict__ body_q) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= S.count) return;
+    const Xf X_wo = shape_world_xform(body_q, S.shape_body, S.shape_transform, S.shapes[i]);
+    const Xf X_wr = shape_world_xform(body_q, S.shape_body, S.shape_transform, S.references[i]);
+    stx(S.transforms + 7 * size_t(i), xmul(xinv(X_wr), X_wo));
+}
+
+NB2_DEV V3 world_gravity(const nb2_sensor_imu_view& S, int world) {  // world -1: the last entry
+    return ld3(S.gravity + 3 * size_t(world >= 0 ? world : S.gravity_count - 1));
+}
+
+// compute_sensor_imu_kernel (sensor_imu.py:16-69), same operation order.
+__global__ void __launch_bounds__(128) sensor_imu_kernel(const nb2_sensor_imu_view S, const float* __restrict__ body_q,
+                                                         const float* __restrict__ body_qd, const float* __restrict__ body_qdd) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= S.count) return;
+    const int s = S.sites[i], b = S.shape_body[s];
+    const Xf Xs = ldx(S.shape_transform + 7 * size_t(s));
+    if (b < 0) {
+        st3(S.accelerometer + 3 * size_t(i), qrot_inv(Xs.q, -world_gravity(S, S.shape_world[s])));
+        st3(S.gyroscope + 3 * size_t(i), V3());
+        return;
+    }
+    const V3 g = world_gravity(S, S.body_world[b]);
+    const float* q = body_q + 7 * size_t(b);
+    const Q4 qb(q[3], q[4], q[5], q[6]);
+    const V3 r = qrot(qb, Xs.p - ld3(S.body_com + 3 * size_t(b)));
+    const V3 w = ld3(body_qd + 6 * size_t(b) + 3);
+    const V3 a_lin = ld3(body_qdd + 6 * size_t(b)), a_ang = ld3(body_qdd + 6 * size_t(b) + 3);
+    const V3 acc = ((a_lin - g) + cross(a_ang, r)) + cross(w, cross(w, r));
+    const Q4 qs = qmul(qb, Xs.q);
+    st3(S.accelerometer + 3 * size_t(i), qrot_inv(qs, acc));
+    st3(S.gyroscope + 3 * size_t(i), qrot_inv(qs, w));
+}
+
 }  // namespace
+
+nb2_status launch_sensor_frame_transform_update(const nb2_sensor_frame_transform_view& S, const float* body_q, cudaStream_t stream) {
+    if (S.count == 0) return NB2_OK;
+    sensor_frame_transform_kernel<<<(S.count + 127) / 128, 128, 0, stream>>>(S, body_q);
+    count_launch(1);
+    NB2_CUDA_CHECK(cudaGetLastError());
+    return NB2_OK;
+}
+
+nb2_status launch_sensor_imu_update(const nb2_sensor_imu_view& S, const float* body_q, const float* body_qd, const float* body_qdd,
+                                    cudaStream_t stream) {
+    if (S.count == 0) return NB2_OK;
+    sensor_imu_kernel<<<(S.count + 127) / 128, 128, 0, stream>>>(S, body_q, body_qd, body_qdd);
+    count_launch(1);
+    NB2_CUDA_CHECK(cudaGetLastError());
+    return NB2_OK;
+}
 
 nb2_status sensor_contact_scratch_bytes(int C, int R, int K, size_t* bytes) {
     SensorScratch s{};

@@ -90,13 +90,31 @@ def _finish(scene: ModelBuilder, device, run_fk=True):
     return model.to(device) if str(device) != "cpu" else model
 
 
-def quadruped_model(world_count: int, device="cpu", seed: int | None = 1, noise: float = 0.02):
+def add_quadruped_sites(quad: ModelBuilder, count: int) -> list[int]:
+    """``count`` sites on the quadruped of :func:`quadruped_builder`, after its shapes: first ``quadruped/imu`` at the base
+    origin, then ``quadruped/<leg>_foot`` at the tip of each shank (0.25 m down its axis), then ``quadruped/site_<k>`` cycling
+    over every body in body order at a small rotated offset.  Returns their shape indices."""
+    body = {label.rsplit("/", 1)[-1]: b for b, label in enumerate(quad.body_label)}
+    placed = [(body["base"], X.transform_identity(), "quadruped/imu")]
+    placed += [(body[f"{leg}_SHANK"], X.transform((0.0, 0.0, -0.25)), f"quadruped/{leg}_foot") for leg in ("LF", "RF", "LH", "RH")]
+    k = 0
+    while len(placed) < count:
+        offset = X.transform((0.01 * (k % 3 + 1), -0.02, 0.015 * (k % 5)), X.quat_from_axis_angle((0.0, 0.0, 1.0), 0.3 * (k + 1)))
+        placed.append((k % quad.body_count, offset, f"quadruped/site_{k}"))
+        k += 1
+    return [quad.add_site(b, xform=xf, label=label) for b, xf, label in placed[:count]]
+
+
+def quadruped_model(world_count: int, device="cpu", seed: int | None = 1, noise: float = 0.02, sites: int = 0):
     """Config 3: ``world_count`` quadrupeds + one global ground plane.
 
     Per-env perturbation (BASELINE.md §3): ``joint_q[7:] += N(0, noise)`` with ``default_rng(seed)``,
-    targets follow; ``seed=None`` keeps every env identical to the stock example.
+    targets follow; ``seed=None`` keeps every env identical to the stock example.  ``sites > 0`` gives every quadruped that many
+    sites (:func:`add_quadruped_sites`); they add no mass and no contact pair, so bodies and joints are those of ``sites=0``.
     """
     quad = quadruped_builder()
+    if sites:
+        add_quadruped_sites(quad, sites)
     scene = ModelBuilder()
     scene.replicate(quad, world_count)
     scene.add_ground_plane(cfg=quad.default_shape_cfg)

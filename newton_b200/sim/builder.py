@@ -80,6 +80,18 @@ class ShapeConfig:
     has_shape_collision: bool = True
     has_particle_collision: bool = True
     is_visible: bool = True
+    is_site: bool = False
+    """A site: a non-colliding, massless reference frame (sensor mounts, tool frames).  Assigning True directly enforces nothing;
+    use :meth:`mark_as_site` or the ``flags`` setter, which apply the site invariants."""
+
+    def mark_as_site(self) -> None:
+        """Make this a site config (reference ``sim/builder.py:709-723``): no shape or particle collision, density 0, collision
+        group 0."""
+        self.is_site = True
+        self.has_shape_collision = False
+        self.has_particle_collision = False
+        self.density = 0.0
+        self.collision_group = 0
 
     @property
     def flags(self) -> int:
@@ -90,7 +102,24 @@ class ShapeConfig:
             f |= ShapeFlags.COLLIDE_SHAPES
         if self.has_particle_collision:
             f |= ShapeFlags.COLLIDE_PARTICLES
+        if self.is_site:
+            f |= ShapeFlags.SITE
         return int(f)
+
+    @flags.setter
+    def flags(self, value: int) -> None:
+        """Reference ``sim/builder.py:736-757``: ``SITE`` applies :meth:`mark_as_site` (whatever collision bits come with it);
+        without ``SITE`` the site fields return to their defaults and the collision bits are taken as given."""
+        self.is_visible = bool(value & ShapeFlags.VISIBLE)
+        if value & ShapeFlags.SITE:
+            self.mark_as_site()
+        else:
+            defaults = type(self)()
+            self.is_site = False
+            self.density = defaults.density
+            self.collision_group = defaults.collision_group
+            self.has_shape_collision = bool(value & ShapeFlags.COLLIDE_SHAPES)
+            self.has_particle_collision = bool(value & ShapeFlags.COLLIDE_PARTICLES)
 
     def copy(self):
         return copy.copy(self)
@@ -234,6 +263,13 @@ class ModelBuilder:
     @property
     def articulation_count(self):
         return len(self.articulation_start)
+
+    @property
+    def default_site_cfg(self) -> ShapeConfig:
+        """A new :class:`ShapeConfig` with the site invariants applied (reference ``sim/builder.py:2381-2395``)."""
+        cfg = ShapeConfig()
+        cfg.mark_as_site()
+        return cfg
 
     @property
     def up_vector(self):
@@ -667,9 +703,25 @@ class ModelBuilder:
         self.body_inv_mass[i] = 1.0 / new_mass if new_mass > 0.0 else 0.0
         self.body_inv_inertia[i] = np.linalg.inv(new_inertia) if new_inertia.any() else new_inertia
 
-    def add_shape(self, *, body, type, xform=None, cfg=None, scale=None, is_static=False, label=None, src=None) -> int:
-        """Reference ``sim/builder.py:6498-6715``."""
-        cfg = cfg or self.default_shape_cfg
+    def add_shape(self, *, body, type, xform=None, cfg=None, scale=None, is_static=False, label=None, src=None, as_site=False) -> int:
+        """Reference ``sim/builder.py:6498-6715``.  ``as_site=True`` adds a site: :attr:`default_site_cfg` without ``cfg``, else a
+        copy of ``cfg`` with the site invariants applied.  A ``cfg`` with ``is_site`` set must already satisfy them."""
+        if cfg is None:
+            cfg = self.default_site_cfg if as_site else self.default_shape_cfg
+        elif as_site:
+            cfg = cfg.copy()
+            cfg.mark_as_site()
+        if cfg.is_site:  # reference sim/builder.py:6608-6633
+            name = label or f"shape_{self.shape_count}"
+            if cfg.has_shape_collision or cfg.has_particle_collision:
+                raise ValueError(f"Site shape '{name}' cannot have collision enabled. Sites must be non-colliding reference points. "
+                                 f"has_shape_collision={cfg.has_shape_collision}, has_particle_collision={cfg.has_particle_collision}")
+            if cfg.density != 0.0:
+                raise ValueError(f"Site shape '{name}' must have zero density. Sites do not contribute to body mass. "
+                                 f"Got density={cfg.density}")
+            if cfg.collision_group != 0:
+                raise ValueError(f"Site shape '{name}' must have collision_group=0. Sites do not participate in collision detection. "
+                                 f"Got collision_group={cfg.collision_group}")
         tf = X.transform_identity() if xform is None else np.asarray(xform, dtype=np.float64)
         type = GeoType(type)
         if type in (GeoType.CONVEX_MESH, GeoType.MESH):
@@ -731,6 +783,14 @@ class ModelBuilder:
             com_body = X.transform_point(tf, c)
             self._update_body_mass(body, m, inertia, com_body, tf[3:])
         return shape
+
+    def add_site(self, body, *, xform=None, type=GeoType.SPHERE, scale=(0.01, 0.01, 0.01), label=None, visible=False) -> int:
+        """A site on ``body`` (-1: fixed in the world) - reference ``sim/builder.py:7381-7436``.  A site is an ordinary shape entry
+        flagged ``SITE``: it adds no mass and takes part in no contact pair; it carries ``VISIBLE`` only with ``visible=True``.
+        ``type`` and ``scale`` only describe how it would be drawn.  Returns its shape index."""
+        cfg = self.default_site_cfg
+        cfg.is_visible = visible
+        return self.add_shape(body=body, type=type, xform=xform, cfg=cfg, scale=scale, label=label)
 
     def add_shape_plane(self, plane=(0.0, 0.0, 1.0, 0.0), *, xform=None, width=10.0, length=10.0, body=-1,
                         cfg=None, label=None) -> int:

@@ -37,6 +37,7 @@ class State:
         self.body_qd: torch.Tensor | None = None  # [B,6] (v_com_world, omega_world)
         self.body_f: torch.Tensor | None = None  # [B,6] (force, torque) at COM, world frame
         self.body_parent_f: torch.Tensor | None = None
+        self.body_qdd: torch.Tensor | None = None  # [B,6] (linear, angular) acceleration; allocated on request, written by no solver here
         self.joint_q: torch.Tensor | None = None  # [coord]
         self.joint_qd: torch.Tensor | None = None  # [dof]
         self.particle_q = None
@@ -50,7 +51,7 @@ class State:
 
     def assign(self, other: "State") -> None:
         """Copy all arrays of ``other`` into this state (reference ``sim/state.py:202-262``)."""
-        for name in ("body_q", "body_qd", "body_f", "body_parent_f", "joint_q", "joint_qd"):
+        for name in ("body_q", "body_qd", "body_f", "body_parent_f", "body_qdd", "joint_q", "joint_qd"):
             src = getattr(other, name)
             dst = getattr(self, name)
             if (src is None) != (dst is None):
@@ -340,6 +341,8 @@ class Model:
             s.body_f = torch.zeros_like(self.body_qd)
             if "body_parent_f" in self._requested_state_attributes:
                 s.body_parent_f = torch.zeros_like(self.body_qd)
+        if "body_qdd" in self._requested_state_attributes:  # allocated even without bodies, as upstream: sensors test it for None
+            s.body_qdd = torch.zeros((self.body_count, 6), dtype=F32, device=self.device)
         if self.joint_count:
             s.joint_q = self.joint_q.clone()
             s.joint_qd = self.joint_qd.clone()
@@ -363,7 +366,7 @@ class Model:
 
     def get_attribute_frequency(self, name: str) -> AttributeFrequency:
         """Frequency of a Model / State / Control attribute (reference ``sim/model.py:2224-2241``)."""
-        if name in _BODY_FIELDS or name in ("body_f", "body_parent_f"):
+        if name in _BODY_FIELDS or name in ("body_f", "body_parent_f", "body_qdd"):
             return AttributeFrequency.BODY
         if name in _JOINT_FIELDS:
             return AttributeFrequency.JOINT
