@@ -194,6 +194,14 @@ typedef struct nb2_featherstone_params {
        path it is opt-in and restricted (articulations of <= 24 dofs); results agree with the default path to ~1e-6 relative, not
        bit for bit. */
     int32_t use_tile_gemm;
+    /* The mass matrix belongs to the solver, not to the model (solver_featherstone.py:190, 284-288, 921).  The caller decides
+       when H and its Cholesky factor are formed - the reference does so on every update_mass_matrix_interval-th step of that
+       solver and on the step after notify_model_changed(BODY_PROPERTIES | JOINT_DOF_PROPERTIES) - and passes form_mass_matrix;
+       nb2_featherstone_step keeps no step count and does not read update_mass_matrix_interval.  mass_matrix_factor is the
+       solver's own device buffer of nb2_featherstone_factor_floats(model) floats: written when form_mass_matrix != 0, read
+       otherwise, so two solvers on one model never share a factor. */
+    int32_t form_mass_matrix;
+    float* mass_matrix_factor;
 } nb2_featherstone_params;
 
 /* Constructor kwargs of reference SolverSemiImplicit (solvers/semi_implicit/solver_semi_implicit.py:72-121) that act on rigid bodies.
@@ -295,6 +303,9 @@ nb2_status nb2_xpbd_update_contacts(nb2_model* model, const nb2_contacts_view* c
 /* Reference SolverBase.integrate_bodies (solvers/solver.py:267-307; kernel :112-170). */
 nb2_status nb2_integrate_bodies(nb2_model* model, const nb2_state_view* state_in, const nb2_state_view* state_out,
                                 float angular_damping, float dt, void* cuda_stream);
+
+/* Size, in floats, of the Cholesky-factor buffer nb2_featherstone_params.mass_matrix_factor points to. */
+int64_t nb2_featherstone_factor_floats(const nb2_model* model);
 
 /* Reference SolverFeatherstone.step (solvers/featherstone/solver_featherstone.py:461-1066). */
 nb2_status nb2_featherstone_step(nb2_model* model, const nb2_featherstone_params* params,

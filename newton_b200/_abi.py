@@ -339,6 +339,8 @@ class FeatherstoneParams(C.Structure):
         ("update_mass_matrix_interval", C.c_int32),
         ("friction_smoothing", C.c_float),
         ("use_tile_gemm", C.c_int32),
+        ("form_mass_matrix", C.c_int32),
+        ("mass_matrix_factor", C.c_void_p),
     ]
 
 

@@ -26,7 +26,7 @@ STATUS = {0: "NB2_OK", 1: "NB2_ERR_INVALID_ARGUMENT", 2: "NB2_ERR_UNSUPPORTED", 
 # every symbol include/newton_b200.h declares
 EXPORTED_SYMBOLS = (
     "nb2_model_create", "nb2_model_destroy", "nb2_model_notify_changed", "nb2_model_rigid_contact_max", "nb2_collide_configure", "nb2_collide", "nb2_collide_speculative", "nb2_contacts_match", "nb2_contacts_sort", "nb2_contacts_import",
-    "nb2_xpbd_step", "nb2_xpbd_update_contacts", "nb2_integrate_bodies", "nb2_featherstone_step", "nb2_semi_implicit_step", "nb2_eval_fk", "nb2_eval_ik", "nb2_eval_fk_masked",
+    "nb2_xpbd_step", "nb2_xpbd_update_contacts", "nb2_integrate_bodies", "nb2_featherstone_factor_floats", "nb2_featherstone_step", "nb2_semi_implicit_step", "nb2_eval_fk", "nb2_eval_ik", "nb2_eval_fk_masked",
     "nb2_eval_jacobian", "nb2_eval_mass_matrix", "nb2_eval_inverse_dynamics_passive", "nb2_eval_inverse_dynamics_force",
     "nb2_sensor_contact_scratch_bytes", "nb2_sensor_contact_update", "nb2_sensor_frame_transform_update", "nb2_sensor_imu_update", "nb2_raycast_refit", "nb2_intersect_ray",
     "nb2_camera_render", "nb2_actuator_step", "nb2_actuator_reset", "nb2_actuator_network_reset", "nb2_actuator_param_gather", "nb2_actuator_param_scatter",
@@ -80,6 +80,8 @@ def lib():
         L.nb2_xpbd_update_contacts.restype = C.c_int
         L.nb2_integrate_bodies.argtypes = [P, C.POINTER(_abi.StateView), C.POINTER(_abi.StateView), C.c_float, C.c_float, P]
         L.nb2_integrate_bodies.restype = C.c_int
+        L.nb2_featherstone_factor_floats.argtypes = [P]
+        L.nb2_featherstone_factor_floats.restype = C.c_int64
         L.nb2_featherstone_step.argtypes = [P, C.POINTER(_abi.FeatherstoneParams), C.POINTER(_abi.StateView),
                                             C.POINTER(_abi.StateView), C.POINTER(_abi.ControlView), C.c_int32, C.c_float, P]
         L.nb2_featherstone_step.restype = C.c_int

@@ -378,6 +378,9 @@ static nb2_status build_tables(nb2_model* m, const nb2_model_desc& d) {
         }
         (void)e;
         m->dev.max_depth = max_depth;
+        m->dev.fs_descendant_free = 0;
+        for (int j = 0; j < J; ++j)
+            if ((jtype[j] == 4 || jtype[j] == 5) && jparent[j] >= 0) m->dev.fs_descendant_free = 1;  // JointType.FREE, DISTANCE
         m->dev.max_env_H = max_env_H;
         m->dev.max_env_arts = max_env_arts;
         int max_dofs = 0, max_coords = 0;
@@ -470,8 +473,6 @@ static nb2_status upload_tables(nb2_model* m) {
     if ((st = upload(h.hb_row_col, m->hb_row_col, &dv.hb_row_col))) return st;
     if ((st = upload(h.joint_desc_mask, m->joint_desc_mask, &dv.joint_desc_mask))) return st;
     if ((st = upload(h.dof_joint, m->dof_joint, &dv.dof_joint))) return st;
-    if ((st = m->fs_L.alloc(std::max<size_t>(size_t(h.env_H_start.back()), 1) * sizeof(float), true))) return st;
-    dv.fs_L = m->fs_L.get<float>();
     if ((st = m->joint_impulse.alloc(std::max<size_t>(size_t(dv.d.joint_count) * 6, 1) * sizeof(float), true))) return st;
     dv.joint_impulse = m->joint_impulse.get<float>();
     if ((st = m->env_contact_count.alloc(E1 * sizeof(int), true))) return st;
@@ -731,6 +732,10 @@ nb2_status nb2_integrate_bodies(nb2_model* model, const nb2_state_view* state_in
     }
     DeviceGuard guard(model->device);
     return launch_integrate_bodies(model, *state_in, *state_out, angular_damping, dt, static_cast<cudaStream_t>(cuda_stream));
+}
+
+int64_t nb2_featherstone_factor_floats(const nb2_model* model) {
+    return model ? std::max<int64_t>(int64_t(model->host.env_H_start.back()), 1) : 0;
 }
 
 nb2_status nb2_featherstone_step(nb2_model* model, const nb2_featherstone_params* params, const nb2_state_view* state_in,

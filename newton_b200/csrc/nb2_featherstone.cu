@@ -579,7 +579,7 @@ featherstone_step_kernel(DevModel M, nb2_featherstone_params P, nb2_state_view s
         const int anj = aj1 - aj0;
         const int ad0 = jqds[aj0], n = jqds[aj1] - ad0;
         float* H = sm.H + M.art_H_start[art];
-        float* Lg = M.fs_L + M.env_H_start[env] + M.art_H_start[art];
+        float* Lg = P.mass_matrix_factor + M.env_H_start[env] + M.art_H_start[art];
         if (update_mass) {
             // H = J^T (M J), lower triangle only (all dense_cholesky reads).  Columns are processed in batches of equal
             // (tree depth of their joint, dof index inside the joint): such joints are never ancestors of one another, so
@@ -825,8 +825,24 @@ featherstone_step_kernel(DevModel M, nb2_featherstone_params P, nb2_state_view s
     }
     __syncwarp(gmask);
     for (int i = l; i < ncoord; i += L) sout.joint_q[c0 + i] = sm.jq[i];
+    // descendant_free_distance_mask (solver_featherstone.py:225-262): FREE / DISTANCE joints with a parent and a non-kinematic child
+    auto descendant_free = [&](int gj) {
+        const int type = jtype[gj];
+        return (type == FJ_FREE || type == FJ_DISTANCE) && jparent[gj] >= 0 && !(d.body_flags[jchild[gj]] & 2);
+    };
+    if (M.fs_descendant_free) {  // their children's pre-step poses (bq as eval_rigid_fk left it) into the dead spatial-inertia block
+        for (int j = l; j < nj; j += L) {
+            if (!descendant_free(j0 + j)) continue;
+            const int child = jchild[j0 + j] - b0;
+            stx(sm.Is + 36 * child, ldx(sm.bq + 7 * child));
+        }
+        __syncwarp(gmask);
+    }
     NB2_PHASE();
-    // ---- eval_fk_with_velocity_conversion: level-parallel; reuses bq (poses) and vs (COM twists) ------------------------
+    // ---- eval_fk_with_velocity_conversion: level-parallel; reuses bq (poses) and vs (COM twists).  A second pass follows the
+    // descendant FREE / DISTANCE correction (solver_featherstone.py:1006-1045): it recomputes every joint, which reproduces the
+    // first pass bit for bit wherever the corrected poses do not reach, i.e. it is the reference's refresh from the first such joint.
+    for (int pass = 0; pass < 2; ++pass) {
     for (int lvl = 0; lvl <= M.max_depth; ++lvl) {
         for (int j = l; j < nj; j += L) {
             const int gj = j0 + j;
@@ -894,6 +910,42 @@ featherstone_step_kernel(DevModel M, nb2_featherstone_params P, nb2_state_view s
             st6(sout.body_qd + 6 * (b0 + child), S6(v_com, w_o));
         }
         __syncwarp(gmask);
+    }
+    if (pass == 1 || !M.fs_descendant_free) break;
+    // correct_free_distance_body_pose_from_world_twist (kernels.py:1914-1930, integrate_body_pose_from_com_twist :1896-1911): the
+    // child moves by its world COM twist from its pre-step pose
+    bool corrected = false;
+    for (int j = l; j < nj; j += L) {
+        if (!descendant_free(j0 + j)) continue;
+        const int child = jchild[j0 + j] - b0;
+        const Xf X_wb = ldx(sm.Is + 36 * child);
+        const V3 com = ld3(d.body_com + 3 * (b0 + child));
+        const V3 x_com = xpoint(X_wb, com);
+        const V3 v = ld3(sm.vs + 6 * child), w = ld3(sm.vs + 6 * child + 3);
+        const Q4 drdt = qscale(qmul(Q4(w.x, w.y, w.z, 0.0f), X_wb.q), 0.5f);
+        const Q4 q_new = qunit(qadd(X_wb.q, qscale(drdt, dt)));
+        const V3 x_com_new = x_com + v * dt;
+        stx(sm.bq + 7 * child, Xf(x_com_new - qrot(q_new, com), q_new));
+        corrected = true;
+    }
+    __syncwarp(gmask);
+    // reconstruct_free_distance_joint_q_from_body_pose (kernels.py:978-1012)
+    for (int j = l; j < nj; j += L) {
+        const int gj = j0 + j;
+        if (!descendant_free(gj)) continue;
+        const Xf X_wpj = xmul(ldx(sm.bq + 7 * (jparent[gj] - b0)), ldx(d.joint_X_p + 7 * gj));
+        const Xf X_wcj = xmul(ldx(sm.bq + 7 * (jchild[gj] - b0)), ldx(d.joint_X_c + 7 * gj));
+        const V3 x_err = qrot_inv(X_wpj.q, X_wcj.p - X_wpj.p);
+        const Q4 q_pc = qmul(qconj(X_wpj.q), X_wcj.q);
+        const float qv[7] = {x_err.x, x_err.y, x_err.z, q_pc.x, q_pc.y, q_pc.z, q_pc.w};
+        const int qs = jqs[gj];
+        for (int k = 0; k < 7; ++k) {
+            sm.jq[qs - c0 + k] = qv[k];
+            sout.joint_q[qs + k] = qv[k];
+        }
+    }
+    if (!__any_sync(gmask, corrected)) break;
+    __syncwarp(gmask);
     }
     // ---- internal -> public joint_qd ------------------------------------------------------------------------------
     for (int j = l; j < nj; j += L) {
@@ -1006,9 +1058,11 @@ nb2_status launch_featherstone_step(nb2_model* m, const nb2_featherstone_params&
     }
     // state_in may be state_out (reference solver_featherstone.py:472): every group finishes reading its environment's inputs
     // (joint_q in the integration pass is the last) before it writes the outputs, and no group touches another environment.
-    const int interval = p.update_mass_matrix_interval > 0 ? p.update_mass_matrix_interval : 1;
-    const int update_mass = (m->featherstone_step_count % interval) == 0;
-    m->featherstone_step_count += 1;
+    if (!p.mass_matrix_factor) {
+        set_error("nb2_featherstone_step: mass_matrix_factor is NULL (the solver's buffer of nb2_featherstone_factor_floats floats)");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    const int update_mass = p.form_mass_matrix != 0;
     switch (m->lanes_per_env) {
         case 8: return launch_fs_L<8>(m, p, in, out, ctl, use_contacts, update_mass, dt, s);
         case 16: return launch_fs_L<16>(m, p, in, out, ctl, use_contacts, update_mass, dt, s);

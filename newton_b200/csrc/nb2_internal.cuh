@@ -115,9 +115,9 @@ struct DevModel {
     const int* joint_depth;            // [J] depth of each joint in its articulation tree (root = 0)
     const unsigned long long* joint_anc_mask;  // [J] bit k set <=> articulation-local joint k is an ancestor-or-self
     const int* art_H_start;            // [A+1] offset of each articulation's nd x nd block inside its env's H storage
-    const int* env_H_start;            // [E+1] global offset of the env's H/L storage (persistent L for update intervals)
-    float* fs_L;                       // persistent Cholesky factors [env_H_start[E]]
+    const int* env_H_start;            // [E+1] global offset of the env's H/L storage (the solver's Cholesky factor: nb2_featherstone_params)
     int max_depth, max_env_dofs, max_env_coords, max_env_H, max_env_arts;
+    int fs_descendant_free;            // some FREE / DISTANCE joint has a parent body: the step's descendant pose correction runs
     // H = J^T M J schedule, derived from the joint tree at nb2_model_create (the kernel indexes, it does not walk bit masks):
     // columns of H are formed in batches of (tree depth, dof number inside the joint) - joints of one batch are never ancestors of
     // one another, so every body and every row sees at most one column per batch
@@ -182,12 +182,11 @@ struct nb2_model {
     nb2::DeviceBuffer env_body_start, env_joint_start, env_shape_start, env_pair_start, env_slot_start, env_art_start, global_shapes, pairs;
     nb2::DeviceBuffer body_joint_start, body_joint_entry, joint_depth, joint_anc_mask, art_H_start, env_H_start;
     nb2::DeviceBuffer art_batch_count, art_hb_body_start, art_hb_row_start, hb_body_col, hb_row_col, joint_desc_mask, dof_joint;
-    nb2::DeviceBuffer fs_L, contact_impulse, joint_impulse, cb;
+    nb2::DeviceBuffer contact_impulse, joint_impulse, cb;
     nb2::DeviceBuffer env_contact_count, env_contact_offset, collide_sync, collide_tile_status;
     nb2::DeviceBuffer collide_tile_count;  // [2][E+1]: dev.collide_tile_count, then dev.collide_tile_offset
     nb2::DeviceBuffer dyn_pairs, env_dyn_count, filter_keys;
     int lanes_per_env = 32;  // sub-warp group width used by the fused kernels
-    int featherstone_step_count = 0;
     // scratch of nb2_contacts_import (allocated on first use, sized by the imported buffer's capacity): keys, sorted keys, indices,
     // sorted indices, capacity words each
     int import_capacity = 0;

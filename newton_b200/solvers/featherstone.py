@@ -12,7 +12,10 @@ from __future__ import annotations
 
 import ctypes as C
 
+import torch
+
 from .. import _abi, _lib
+from ..sim.enums import ModelFlags
 from .solver import SolverBase
 
 
@@ -28,6 +31,19 @@ class SolverFeatherstone(SolverBase):
         self.friction_smoothing = friction_smoothing
         self.use_tile_gemm = use_tile_gemm
         self.fuse_cholesky = fuse_cholesky
+        # the mass-matrix schedule and the Cholesky factor the steps in between reuse belong to this solver (solver_featherstone.py:
+        # 189-190): a second solver on the same model starts its own count and never reads this one's factor
+        self._step = 0
+        self._mass_matrix_dirty = False
+        self._factor = torch.empty(int(_lib.lib().nb2_featherstone_factor_floats(self._native.handle)), dtype=torch.float32,
+                                   device=torch.device("cuda", self._native.device_index))
+
+    def notify_model_changed(self, flags: int) -> None:
+        """Reference ``solver_featherstone.py:284-288``: body or dof properties (masses, inertias, kinematic flags, armature)
+        enter the mass matrix, so the next step forms it whatever ``update_mass_matrix_interval`` says."""
+        super().notify_model_changed(flags)
+        if int(flags) & (ModelFlags.BODY_PROPERTIES | ModelFlags.JOINT_DOF_PROPERTIES):
+            self._mass_matrix_dirty = True
 
     def step(self, state_in, state_out, control, contacts, dt: float) -> None:
         """Advance by ``dt`` (reference ``solver_featherstone.py:461-1066``): writes ``state_out.joint_q/joint_qd/
@@ -37,10 +53,14 @@ class SolverFeatherstone(SolverBase):
         if control is None:
             control = model.control(clone_variables=False)
         use_contacts = 1 if self._prepare_contacts(contacts) else 0
+        form = self._mass_matrix_dirty or self._step % max(int(self.update_mass_matrix_interval), 1) == 0
         p = _abi.FeatherstoneParams(self.angular_damping, int(self.update_mass_matrix_interval), self.friction_smoothing,
-                                    1 if self.use_tile_gemm else 0)
+                                    1 if self.use_tile_gemm else 0, 1 if form else 0, self._factor.data_ptr())
         st = _lib.lib().nb2_featherstone_step(
             self._native.handle, C.byref(p), C.byref(_abi.state_view(state_in, model)), C.byref(_abi.state_view(state_out, model)),
             C.byref(_abi.control_view(control, model)), use_contacts, C.c_float(dt), _lib.current_stream_ptr(model),
         )
         _lib.check(st, "nb2_featherstone_step")
+        if form:
+            self._mass_matrix_dirty = False
+        self._step += 1

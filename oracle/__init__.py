@@ -254,8 +254,10 @@ class SolverFeatherstone:
         """SolverBase.reset (solvers/solver.py:344-375): no-op for Featherstone."""
 
     def notify_model_changed(self, flags):
-        """SolverBase.notify_model_changed (solvers/solver.py:394-429): the kernels read the Model arrays on every step."""
+        """SolverFeatherstone.notify_model_changed (solver_featherstone.py:284-288): the kernels read the Model arrays on every
+        step; BODY_PROPERTIES / JOINT_DOF_PROPERTIES also make the next step form the mass matrix."""
         self._desc = _abi.model_desc(self.model)
+        lib().orc_featherstone_notify_changed(self._h, C.c_int(int(flags)))
 
     def step(self, state_in, state_out, control, contacts, dt):
         if control is None:

@@ -231,7 +231,7 @@ void orc_xpbd_update_contacts(const nb2_contacts_view* c, const float* contact_i
         for (int k = 0; k < 6; ++k) c->force[6 * tid + k] = tid < count ? contact_impulse[6 * tid + k] * inv_dt : 0.0f;
 }
 
-// SolverFeatherstone keeps cross-step state (step counter, cached H / L): one handle per solver instance.
+// SolverFeatherstone keeps cross-step state (step counter, mass-matrix dirty flag, cached H / L): one handle per solver instance.
 void* orc_featherstone_new(void) { return new FsScratch(); }
 void orc_featherstone_free(void* h) { delete static_cast<FsScratch*>(h); }
 void orc_featherstone_step(void* h, const nb2_model_desc* m, const nb2_featherstone_params* p, const nb2_state_view* state_in,
@@ -239,6 +239,7 @@ void orc_featherstone_step(void* h, const nb2_model_desc* m, const nb2_featherst
                            float dt) {
     featherstone_step(*static_cast<FsScratch*>(h), *m, *p, *state_in, *state_out, *control, contacts, dt);
 }
+void orc_featherstone_notify_changed(void* h, int flags) { fs_notify_model_changed(*static_cast<FsScratch*>(h), flags); }
 
 // ---- unit-level hooks for known-answer tests ------------------------------------------------------
 // One analytic pair: types/scales/transforms in, up to 4 (distance, position) + normal out.

@@ -144,9 +144,23 @@ struct FsScratch {  // the per-solver aux arrays of solver_featherstone.py:361-4
     std::vector<float> joint_S_s, joint_qd_in, joint_qd_out, joint_f_internal, joint_tau, joint_qdd;
     std::vector<float> J, M, P, H, L;
     std::vector<int> J_start, M_start, H_start;
+    std::vector<float> body_q_prev;  // _featherstone_body_q_prev (solver_featherstone.py:514-516)
     int step = 0;
+    bool mass_matrix_dirty = false;  // _mass_matrix_dirty (solver_featherstone.py:190, 284-288)
     bool init = false;
 };
+
+// notify_model_changed (solver_featherstone.py:284-288): body or dof properties changed -> form H on the next step
+enum { MODEL_JOINT_DOF_PROPERTIES = 1 << 1, MODEL_BODY_PROPERTIES = 1 << 2 };  // ModelFlags (sim/enums.py:19-22)
+inline void fs_notify_model_changed(FsScratch& s, int flags) {
+    if (flags & (MODEL_JOINT_DOF_PROPERTIES | MODEL_BODY_PROPERTIES)) s.mass_matrix_dirty = true;
+}
+
+// descendant_free_distance_mask (solver_featherstone.py:225-262): FREE / DISTANCE joints with a parent and a non-kinematic child
+inline bool descendant_free_distance(const nb2_model_desc& m, int j) {
+    const int t = m.joint_type[j];
+    return (t == JT_FREE || t == JT_DISTANCE) && m.joint_parent[j] >= 0 && !(m.body_flags[m.joint_child[j]] & BODY_KINEMATIC);
+}
 
 // kernels.py:142-238
 inline transform jcalc_transform(const nb2_model_desc& m, int type, int axis_start, int lin, int ang, const float* joint_q, int q_start) {
@@ -366,6 +380,11 @@ inline void featherstone_step(FsScratch& s, const nb2_model_desc& m, const nb2_f
             X_wc.store(sin.body_q + 7 * child);
             X_sm.store(s.body_q_com.data() + 7 * child);
         }
+    // the pre-step poses the descendant FREE / DISTANCE correction integrates from: state_in.body_q as eval_rigid_fk left it, copied
+    // because a step in place overwrites it (solver_featherstone.py:481, 514-516)
+    bool any_descendant = false;
+    for (int j = 0; j < J; ++j) any_descendant = any_descendant || descendant_free_distance(m, j);
+    if (any_descendant) s.body_q_prev.assign(sin.body_q, sin.body_q + size_t(B) * 7);
     // ---- body_f_ext = body_f (+ FREE/DISTANCE joint_f as COM wrenches, kernels.py:893-921)
     std::memcpy(s.body_f_ext.data(), sin.body_f, size_t(B) * 6 * sizeof(float));
     for (int j = 0; j < J; ++j) {
@@ -501,7 +520,8 @@ inline void featherstone_step(FsScratch& s, const nb2_model_desc& m, const nb2_f
             }
     }
     // ---- mass matrix: J, M, P = M J, H = J^T P, L = chol(H + diag(armature)) (solver_featherstone.py:767-921)
-    if (s.step % (p.update_mass_matrix_interval > 0 ? p.update_mass_matrix_interval : 1) == 0) {
+    if (s.mass_matrix_dirty || s.step % (p.update_mass_matrix_interval > 0 ? p.update_mass_matrix_interval : 1) == 0) {
+        s.mass_matrix_dirty = false;
         for (int a = 0; a < A; ++a) {
             int j0 = m.articulation_start[a], j1 = art_end(a), nj = j1 - j0;
             int d0 = m.joint_qd_start[j0], nd = m.joint_qd_start[j1] - d0;
@@ -645,9 +665,9 @@ inline void featherstone_step(FsScratch& s, const nb2_model_desc& m, const nb2_f
             for (int i = m.joint_q_start[j]; i < m.joint_q_start[j + 1]; ++i) sout.joint_q[i] = sin.joint_q[i];
             for (int i = m.joint_qd_start[j]; i < m.joint_qd_start[j + 1]; ++i) s.joint_qd_out[i] = s.joint_qd_in[i];
         }
-    // ---- eval_fk_with_velocity_conversion (kernels.py:1987-2149) -> state_out.body_q / body_qd
-    for (int a = 0; a < A; ++a)
-        for (int i = m.articulation_start[a]; i < art_end(a); ++i) {
+    // ---- eval_fk_with_velocity_conversion (kernels.py:1987-2149) -> state_out.body_q / body_qd, joints [start, end) of one articulation
+    auto fk_with_velocity_conversion = [&](int start, int end) {
+        for (int i = start; i < end; ++i) {
             int parent = m.joint_parent[i], child = m.joint_child[i], type = m.joint_type[i];
             int qs = m.joint_q_start[i], qds = m.joint_qd_start[i];
             int lin = m.joint_dof_dim[2 * i], ang = m.joint_dof_dim[2 * i + 1];
@@ -709,6 +729,42 @@ inline void featherstone_step(FsScratch& s, const nb2_model_desc& m, const nb2_f
             vec3 v_com = cross(w_o, transform_vector(X_wc, load3(m.body_com + 3 * child))) + v_o;
             spatial(v_com, w_o).store(sout.body_qd + 6 * child);
         }
+    };
+    for (int a = 0; a < A; ++a) fk_with_velocity_conversion(m.articulation_start[a], art_end(a));
+    if (any_descendant) {
+        // correct_free_distance_body_pose_from_world_twist (kernels.py:1914-1930, integrate_body_pose_from_com_twist :1896-1911):
+        // a descendant FREE / DISTANCE child moves by its world COM twist from its pre-step pose
+        for (int j = 0; j < J; ++j) {
+            if (!descendant_free_distance(m, j)) continue;
+            int child = m.joint_child[j];
+            transform X_wb = transform::load(s.body_q_prev.data() + 7 * child);
+            vec3 com = load3(m.body_com + 3 * child);
+            vec3 x_com = transform_point(X_wb, com);
+            spatial qd = spatial::load(sout.body_qd + 6 * child);
+            quat drdt = quat(qd.bot, 0.0f) * X_wb.q * 0.5f;
+            quat q_new = normalize(X_wb.q + drdt * dt);
+            vec3 x_com_new = x_com + qd.top * dt;
+            transform(x_com_new - quat_rotate(q_new, com), q_new).store(sout.body_q + 7 * child);
+        }
+        // reconstruct_free_distance_joint_q_from_body_pose (kernels.py:978-1012)
+        for (int j = 0; j < J; ++j) {
+            if (!descendant_free_distance(m, j)) continue;
+            int parent = m.joint_parent[j], child = m.joint_child[j];
+            transform X_wpj = transform::load(sout.body_q + 7 * parent) * transform::load(m.joint_X_p + 7 * j);
+            transform X_wcj = transform::load(sout.body_q + 7 * child) * transform::load(m.joint_X_c + 7 * j);
+            vec3 x_err_c = quat_rotate_inv(X_wpj.q, X_wcj.p - X_wpj.p);
+            quat q_pc = quat_inverse(X_wpj.q) * X_wcj.q;
+            transform(x_err_c, q_pc).store(sout.joint_q + m.joint_q_start[j]);
+        }
+        // eval_fk_with_velocity_conversion_from_joint_starts (kernels.py:2221-2265, 2332-2368): each articulation again from its
+        // first such joint
+        for (int a = 0; a < A; ++a)
+            for (int i = m.articulation_start[a]; i < art_end(a); ++i)
+                if (descendant_free_distance(m, i)) {
+                    fk_with_velocity_conversion(i, art_end(a));
+                    break;
+                }
+    }
     // ---- internal -> public qd (kernels.py:1015-1066)
     for (int j = 0; j < J; ++j) {
         int qd0 = m.joint_qd_start[j], qd1 = m.joint_qd_start[j + 1], t = m.joint_type[j];
