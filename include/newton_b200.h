@@ -232,6 +232,12 @@ nb2_status nb2_model_notify_changed(nb2_model* model, const nb2_model_desc* desc
  * sim/collide.py:553-652 gives an upper bound; this is the exact per-pair bound used by the blocks). */
 int32_t nb2_model_rigid_contact_max(const nb2_model* model);
 
+/* Diagnostics: what the last nb2_xpbd_step launch on this model chose.  out[0] = 1 when every environment's body and joint
+ * constants equal environment 0's (template mode: one copy per CTA in shared memory), out[1] = contacts per environment whose
+ * constants are cached in shared memory, out[2] = contact records per environment, out[3] = dynamic shared memory per CTA (bytes).
+ * All zero before the first step. */
+nb2_status nb2_xpbd_plan_info(const nb2_model* model, int32_t* out);
+
 /* --- hot path ------------------------------------------------------------------------------- */
 
 /* Broad-phase selection of reference CollisionPipeline(broad_phase=..., shape_pairs_max=..., include_static_kinematic_pairs=...)

@@ -25,7 +25,7 @@ STATUS = {0: "NB2_OK", 1: "NB2_ERR_INVALID_ARGUMENT", 2: "NB2_ERR_UNSUPPORTED", 
 
 # every symbol include/newton_b200.h declares
 EXPORTED_SYMBOLS = (
-    "nb2_model_create", "nb2_model_destroy", "nb2_model_notify_changed", "nb2_model_rigid_contact_max", "nb2_collide_configure", "nb2_collide", "nb2_collide_speculative", "nb2_contacts_match", "nb2_contacts_sort", "nb2_contacts_import",
+    "nb2_model_create", "nb2_model_destroy", "nb2_model_notify_changed", "nb2_model_rigid_contact_max", "nb2_xpbd_plan_info", "nb2_collide_configure", "nb2_collide", "nb2_collide_speculative", "nb2_contacts_match", "nb2_contacts_sort", "nb2_contacts_import",
     "nb2_xpbd_step", "nb2_xpbd_update_contacts", "nb2_integrate_bodies", "nb2_featherstone_factor_floats", "nb2_featherstone_step", "nb2_semi_implicit_step", "nb2_eval_fk", "nb2_eval_ik", "nb2_eval_fk_masked",
     "nb2_eval_jacobian", "nb2_eval_mass_matrix", "nb2_eval_inverse_dynamics_passive", "nb2_eval_inverse_dynamics_force",
     "nb2_sensor_contact_scratch_bytes", "nb2_sensor_contact_update", "nb2_sensor_frame_transform_update", "nb2_sensor_imu_update", "nb2_raycast_refit", "nb2_intersect_ray",
@@ -61,6 +61,8 @@ def lib():
         L.nb2_model_notify_changed.restype = C.c_int
         L.nb2_model_rigid_contact_max.argtypes = [P]
         L.nb2_model_rigid_contact_max.restype = C.c_int32
+        L.nb2_xpbd_plan_info.argtypes = [P, C.POINTER(C.c_int32)]
+        L.nb2_xpbd_plan_info.restype = C.c_int
         L.nb2_collide_configure.argtypes = [P, C.c_int32, C.c_int32, C.c_int32]
         L.nb2_collide_configure.restype = C.c_int
         L.nb2_collide.argtypes = [P, P, C.POINTER(_abi.ContactsView), P]
@@ -206,6 +208,12 @@ class NativeModel:
               "nb2_collide_configure")
         self.rigid_contact_max = int(lib().nb2_model_rigid_contact_max(self.handle))
         self.contact_stamp += 1  # whatever sat in the old blocks is gone
+
+    def xpbd_plan_info(self) -> dict:
+        """What the last XPBD step launch chose (``nb2_xpbd_plan_info``): template mode, cached contacts, contact records, shared bytes."""
+        out = (C.c_int32 * 4)()
+        check(lib().nb2_xpbd_plan_info(self.handle, out), "nb2_xpbd_plan_info")
+        return {"template": bool(out[0]), "contact_cache": int(out[1]), "contact_cap": int(out[2]), "smem_bytes": int(out[3])}
 
     def notify_model_changed(self, flags: int):
         self.desc = _abi.model_desc(self.model)

@@ -570,6 +570,72 @@ static nb2_status configure_broad_phase(nb2_model* m, int mode, int max_pairs, b
     return NB2_OK;
 }
 
+// XPBD template mode (nb2_xpbd.cu): every environment has environment 0's bodies and joints with bit-identical constants -
+// com, inverse mass, inertia, inverse inertia and flags; type, enabled flag, dof counts, frames, axes, limits, target gains, and
+// parent, child, dof and target offsets relative to the environment's first body / joint - so that xpbd_step_kernel may read them
+// from one copy per CTA.  The kernels read the Model arrays live, so a change of any of them must be followed by
+// nb2_model_notify_changed, which runs this again.
+static nb2_status detect_xpbd_template(nb2_model* m) {
+    m->xpbd_template = false;
+    const nb2_model_desc& d = m->dev.d;
+    const HostTables& h = m->host;
+    const int E = m->dev.env_count, B = d.body_count, J = d.joint_count, D = d.joint_dof_count;
+    if (E < 1 || B == 0) return NB2_OK;
+    // a model without some of these arrays is not stepped by XPBD: nothing to share
+    if (!d.body_com || !d.body_inv_mass || !d.body_inertia || !d.body_inv_inertia || !d.body_flags) return NB2_OK;
+    if (J > 0 && (!d.joint_type || !d.joint_enabled || !d.joint_parent || !d.joint_child || !d.joint_X_p || !d.joint_X_c ||
+                  !d.joint_qd_start || !d.joint_target_q_start || !d.joint_dof_dim ||
+                  (D > 0 && (!d.joint_axis || !d.joint_limit_lower || !d.joint_limit_upper || !d.joint_target_ke || !d.joint_target_kd))))
+        return NB2_OK;
+    std::vector<float> com, inv_mass, inertia, inv_inertia, X_p, X_c, axis, lo, up, ke, kd;
+    std::vector<int> flags, type, parent, child, qd_start, tq_start, dof_dim;
+    std::vector<uint8_t> enabled;
+    nb2_status st;
+    if ((st = fetch(d.body_com, size_t(B) * 3, com)) || (st = fetch(d.body_inv_mass, size_t(B), inv_mass)) ||
+        (st = fetch(d.body_inertia, size_t(B) * 9, inertia)) || (st = fetch(d.body_inv_inertia, size_t(B) * 9, inv_inertia)) ||
+        (st = fetch(d.body_flags, size_t(B), flags)))
+        return st;
+    if (J > 0 &&
+        ((st = fetch(d.joint_type, size_t(J), type)) || (st = fetch(d.joint_enabled, size_t(J), enabled)) ||
+         (st = fetch(d.joint_parent, size_t(J), parent)) || (st = fetch(d.joint_child, size_t(J), child)) ||
+         (st = fetch(d.joint_X_p, size_t(J) * 7, X_p)) || (st = fetch(d.joint_X_c, size_t(J) * 7, X_c)) ||
+         (st = fetch(d.joint_qd_start, size_t(J) + 1, qd_start)) || (st = fetch(d.joint_target_q_start, size_t(J), tq_start)) ||
+         (st = fetch(d.joint_dof_dim, size_t(J) * 2, dof_dim)) || (st = fetch(d.joint_axis, size_t(D) * 3, axis)) ||
+         (st = fetch(d.joint_limit_lower, size_t(D), lo)) || (st = fetch(d.joint_limit_upper, size_t(D), up)) ||
+         (st = fetch(d.joint_target_ke, size_t(D), ke)) || (st = fetch(d.joint_target_kd, size_t(D), kd))))
+        return st;
+    // n records of w elements at a and b are equal word for word
+    auto same = [](const auto& v, size_t w, size_t a, size_t b, size_t n) {
+        return n == 0 || std::memcmp(&v[a * w], &v[b * w], n * w * sizeof(v[0])) == 0;
+    };
+    const int tb0 = h.env_body_start[0], nb = h.env_body_start[1] - tb0, tj0 = h.env_joint_start[0], nj = h.env_joint_start[1] - tj0;
+    const int td0 = J > 0 ? qd_start[tj0] : 0, nd = J > 0 ? qd_start[tj0 + nj] - td0 : 0;
+    for (int e = 1; e < E; ++e) {
+        const int b0 = h.env_body_start[e], j0 = h.env_joint_start[e];
+        if (h.env_body_start[e + 1] - b0 != nb || h.env_joint_start[e + 1] - j0 != nj) return NB2_OK;
+        if (!same(com, 3, b0, tb0, nb) || !same(inv_mass, 1, b0, tb0, nb) || !same(inertia, 9, b0, tb0, nb) ||
+            !same(inv_inertia, 9, b0, tb0, nb) || !same(flags, 1, b0, tb0, nb))
+            return NB2_OK;
+        if (nj == 0) continue;
+        if (!same(type, 1, j0, tj0, nj) || !same(enabled, 1, j0, tj0, nj) || !same(dof_dim, 2, j0, tj0, nj) ||
+            !same(X_p, 7, j0, tj0, nj) || !same(X_c, 7, j0, tj0, nj))
+            return NB2_OK;
+        const int d0 = qd_start[j0];
+        if (qd_start[j0 + nj] - d0 != nd) return NB2_OK;
+        for (int k = 0; k < nj; ++k) {
+            const int p = parent[j0 + k], tp = parent[tj0 + k];
+            if ((p < 0 ? -1 : p - b0) != (tp < 0 ? -1 : tp - tb0) || child[j0 + k] - b0 != child[tj0 + k] - tb0 ||
+                qd_start[j0 + k] - d0 != qd_start[tj0 + k] - td0 || tq_start[j0 + k] - tq_start[j0] != tq_start[tj0 + k] - tq_start[tj0])
+                return NB2_OK;
+        }
+        if (!same(axis, 3, d0, td0, nd) || !same(lo, 1, d0, td0, nd) || !same(up, 1, d0, td0, nd) || !same(ke, 1, d0, td0, nd) ||
+            !same(kd, 1, d0, td0, nd))
+            return NB2_OK;
+    }
+    m->xpbd_template = true;
+    return NB2_OK;
+}
+
 }  // namespace nb2
 
 using namespace nb2;
@@ -587,6 +653,7 @@ nb2_status nb2_model_create(const nb2_model_desc* desc, int32_t device, nb2_mode
     m->device = device;
     nb2_status st = build_tables(m.get(), *desc);
     if (st == NB2_OK) st = upload_tables(m.get());
+    if (st == NB2_OK) st = detect_xpbd_template(m.get());
     if (st != NB2_OK) return st;
     m->explicit_max_env_contacts = m->max_env_contacts;
     m->explicit_has_convex_pairs = m->has_convex_pairs;
@@ -616,7 +683,17 @@ nb2_status nb2_model_notify_changed(nb2_model* model, const nb2_model_desc* desc
         set_error("nb2_model_notify_changed: topology changed; create a new nb2_model");
         return NB2_ERR_UNSUPPORTED;
     }
+    DeviceGuard guard(model->device);
     model->dev.d = *desc;
+    return detect_xpbd_template(model);
+}
+
+nb2_status nb2_xpbd_plan_info(const nb2_model* model, int32_t* out) {
+    if (!model || !out) {
+        set_error("nb2_xpbd_plan_info: NULL argument");
+        return NB2_ERR_INVALID_ARGUMENT;
+    }
+    for (int k = 0; k < 4; ++k) out[k] = model->xpbd_last_plan[k];
     return NB2_OK;
 }
 

@@ -218,6 +218,10 @@ struct nb2_model {
     int max_env_contacts = 0;       // max over envs of the sum of the pairs' own contact maxima (<= 4 analytic, <= 5 manifold)
     bool contacts_imported = false; // the contact blocks hold an imported foreign buffer (any count up to the slot range)
     float xpbd_impulse_dt = 0.0f;  // dt of the last nb2_xpbd_step that accumulated contact impulses (0 = none yet)
+    // every environment's XPBD body and joint constants equal environment 0's, in environment-relative indices (checked at
+    // nb2_model_create and nb2_model_notify_changed): xpbd_step_kernel holds one copy of them per CTA
+    bool xpbd_template = false;
+    int xpbd_last_plan[4] = {};  // nb2_xpbd_plan_info: template mode, contact cache, contact records, shared bytes of the last launch
 };
 
 namespace nb2 {

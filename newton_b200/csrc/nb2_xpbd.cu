@@ -30,7 +30,10 @@ enum { BODY_KINEMATIC = 2 };
 // shared-memory body record (floats): odd stride -> consecutive bodies hit different banks.  BR_WCOM is the world centre of mass
 // xpoint(pose, com) of the pose in BR_Q, formed with the very same expression wherever the pose is written (integrate, apply_delta),
 // so that the contact and joint rows and the next apply_delta read it instead of rotating com again.  Word 38 is padding.
-enum { BR_Q = 0, BR_QD = 7, BR_COM = 13, BR_INVM = 16, BR_INVI = 17, BR_I = 26, BR_WCOM = 35, BR_SIZE = 39 };
+// The state (pose, twist, world centre of mass) comes first: in template mode an environment's record is only its
+// first BR_DYN words, and the constants (com, inverse mass, inertia) are read at the same offsets from the CTA's template record
+// (xpbd_step_body<..., TPL = true>).
+enum { BR_Q = 0, BR_QD = 7, BR_WCOM = 13, BR_COM = 16, BR_INVM = 19, BR_INVI = 20, BR_I = 29, BR_SIZE = 39, BR_DYN = 17 };
 enum { DR_SIZE = 13 };  // delta record: lin_a, ang_a, lin_b, ang_b, active
 enum { XF_JOINT_CACHE = 1, XF_TMA = 2, XF_PHASE_SYNC = 4, XF_PHASE_SYNC_FINE = 8 };  // kernel flags
 // per-contact constants of the Jacobi loop, staged once per substep: point0, point1, normal, margin0 + margin1, the three friction
@@ -82,34 +85,37 @@ struct BodyView {
     Xf X;
     V3 wcom;  // xpoint(X, com)
     float inv_m;
-    const float* rec;  // shared-memory record (inverse inertia is read from it on demand); nullptr = the static world
+    const float* rec;   // shared-memory state record; nullptr = the static world
+    const float* crec;  // its constants (the inverse inertia is read on demand): rec itself, or the CTA's template record
     V3 v, w;
 };
 
-NB2_DEV BodyView load_body(const float* rec) {
+NB2_DEV BodyView load_body(const float* rec, const float* crec) {
     BodyView b;
     b.X = ldx(rec + BR_Q);
     b.v = ld3(rec + BR_QD);
     b.w = ld3(rec + BR_QD + 3);
     b.wcom = ld3(rec + BR_WCOM);
-    b.inv_m = rec[BR_INVM];
+    b.inv_m = crec[BR_INVM];
     b.rec = rec;
+    b.crec = crec;
     return b;
 }
 NB2_DEV BodyView static_body() {  // body index -1: the world
     BodyView b;
     b.inv_m = 0.f;
     b.rec = nullptr;
+    b.crec = nullptr;
     return b;
 }
 
 // r^T I^-1 r with r = ang rotated into the body frame: the angular term of the generalized inverse mass.  For the static
 // world the reference multiplies by a zero inverse inertia; the sum is +-0 and adding it leaves the denominator unchanged.
-NB2_HELPER float ang_inv_mass(const float* rec, V3 ang) {
+NB2_HELPER float ang_inv_mass(const float* rec, const float* crec, V3 ang) {
     if (rec == nullptr) return 0.0f;
     const Q4 q(rec[BR_Q + 3], rec[BR_Q + 4], rec[BR_Q + 5], rec[BR_Q + 6]);
     const V3 r = qrot_inv(q, ang);
-    return dot(r, mv(ldm(rec + BR_INVI), r));
+    return dot(r, mv(ldm(crec + BR_INVI), r));
 }
 
 // Exactness of the reduced expressions below.  Every value these helpers feed reaches the outputs either through a sum that starts
@@ -125,15 +131,15 @@ NB2_DEV float generalized_inv_mass(const BodyView& a, const BodyView& b, V3 lin_
     float denom = 0.0f;
     if (a.rec != nullptr) denom += len2(lin_a) * a.inv_m;
     if (b.rec != nullptr) denom += len2(lin_b) * b.inv_m;
-    denom += ang_inv_mass(a.rec, ang_a);
-    denom += ang_inv_mass(b.rec, ang_b);
+    denom += ang_inv_mass(a.rec, a.crec, ang_a);
+    denom += ang_inv_mass(b.rec, b.crec, ang_b);
     return denom;
 }
 // the same for a purely angular row (zero linear parts: len2(0) * inv_m = +0 for both bodies)
 NB2_DEV float angular_inv_mass(const BodyView& a, const BodyView& b, V3 ang_a, V3 ang_b) {
     float denom = 0.0f;
-    denom += ang_inv_mass(a.rec, ang_a);
-    denom += ang_inv_mass(b.rec, ang_b);
+    denom += ang_inv_mass(a.rec, a.crec, ang_a);
+    denom += ang_inv_mass(b.rec, b.crec, ang_b);
     return denom;
 }
 NB2_DEV float contact_delta(float err, float denom, float relaxation, float dt) {
@@ -209,22 +215,44 @@ struct Deltas {
 // Per-joint quantities that do not change over the Jacobi iterations, staged once per substep in shared memory when it
 // fits next to the body records without costing a resident CTA: the two joint frames and the angular AxisSetup.
 // ... and the joint's integer header (type, enabled, dof counts, child / parent, axis and target offsets), so the
-// iteration loop issues no global loads for joint data at all.
-enum { JC_XP = 0, JC_XC = 7, JC_ANG = 14, JC_HDR = 32, JC_CHILD = 33, JC_PARENT = 34, JC_AXIS = 35, JC_TARGET = 36,
-       JC_SIZE = 37 };  // odd stride: consecutive joints (lanes) hit different banks
+// iteration loop issues no global loads for joint data at all.  JC_ANG holds the model part of the angular AxisSetup (limits,
+// stiffness, damping), JC_TGT its Control part (target_pos, target_vel).  In template mode the CTA keeps one such record per joint
+// of its first environment, and each environment keeps only its own JC_TGT words (JT_SIZE, odd stride).
+enum { JC_XP = 0, JC_XC = 7, JC_ANG = 14, JC_TGT = 26, JC_HDR = 32, JC_CHILD = 33, JC_PARENT = 34, JC_AXIS = 35, JC_TARGET = 36,
+       JC_SIZE = 37, JT_SIZE = 7 };  // odd stride: consecutive joints (lanes) hit different banks
 NB2_DEV int jc_int(const float* jc, int k) { return reinterpret_cast<const int*>(jc)[k]; }
-NB2_DEV void store_axis_setup(float* p, const AxisSetup& s) {
-    st3(p, s.lim_lo); st3(p + 3, s.lim_up); st3(p + 6, s.target_pos); st3(p + 9, s.stiffness); st3(p + 12, s.target_vel); st3(p + 15, s.damping);
+NB2_DEV void store_axis_targets(float* t, const AxisSetup& s) {
+    st3(t, s.target_pos); st3(t + 3, s.target_vel);
 }
-NB2_DEV AxisSetup load_axis_setup(const float* p) {
+NB2_DEV AxisSetup load_axis_setup(const float* c, const float* t) {
     AxisSetup s;
-    s.lim_lo = ld3(p); s.lim_up = ld3(p + 3); s.target_pos = ld3(p + 6); s.stiffness = ld3(p + 9); s.target_vel = ld3(p + 12); s.damping = ld3(p + 15);
+    s.lim_lo = ld3(c); s.lim_up = ld3(c + 3); s.stiffness = ld3(c + 6); s.damping = ld3(c + 9);
+    s.target_pos = ld3(t); s.target_vel = ld3(t + 3);
     return s;
 }
+// the joint cache record of joint gj (global index)
+NB2_GPU void fill_joint_cache(const nb2_model_desc& d, const nb2_control_view& ctl, float* jc, int gj) {
+    const int lin_count = d.joint_dof_dim[2 * gj], ang_count = d.joint_dof_dim[2 * gj + 1];
+    const int axis_start = d.joint_qd_start[gj], target_start = d.joint_target_q_start[gj];
+    stx(jc + JC_XP, ldx(d.joint_X_p + 7 * gj));
+    stx(jc + JC_XC, ldx(d.joint_X_c + 7 * gj));
+    const AxisSetup s = gather_axes(d, ctl, axis_start, target_start, lin_count, ang_count);
+    st3(jc + JC_ANG, s.lim_lo); st3(jc + JC_ANG + 3, s.lim_up); st3(jc + JC_ANG + 6, s.stiffness); st3(jc + JC_ANG + 9, s.damping);
+    store_axis_targets(jc + JC_TGT, s);
+    jc[JC_HDR] = __int_as_float(d.joint_type[gj] | (d.joint_enabled[gj] ? 16 : 0) | (lin_count << 8) | (ang_count << 12));
+    jc[JC_CHILD] = __int_as_float(d.joint_child[gj]);
+    jc[JC_PARENT] = __int_as_float(d.joint_parent[gj]);
+    jc[JC_AXIS] = __int_as_float(axis_start);
+    jc[JC_TARGET] = __int_as_float(target_start);
+}
 
-// lin_alpha_dt / ang_alpha_dt: P.joint_linear_compliance / dt and P.joint_angular_compliance / dt, formed once per substep
+// lin_alpha_dt / ang_alpha_dt: P.joint_linear_compliance / dt and P.joint_angular_compliance / dt, formed once per substep.
+// Body records: state at bodies + i * bstride, constants at cbodies + i * BR_SIZE.  jc: the joint's cache record (nullptr: read the
+// Model), jt: its JC_TGT words.  tpl: jc belongs to the template environment, whose first body is body0; its axis and target
+// offsets are not this joint's, so the paths that index the Model by them read this joint's own from the Model.
 NB2_DEV bool solve_joint(const nb2_model_desc& d, const nb2_control_view& ctl, const nb2_xpbd_params& P, int j, int body0,
-                         const float* bodies, const float* jc, float dt, float lin_alpha_dt, float ang_alpha_dt, Deltas& out) {
+                         const float* bodies, int bstride, const float* cbodies, const float* jc, const float* jt, bool tpl, float dt,
+                         float lin_alpha_dt, float ang_alpha_dt, Deltas& out) {
     // header: bits 0-3 type, bit 4 enabled, bits 8-11 / 12-15 linear / angular dof counts
     const int hdr = jc ? jc_int(jc, JC_HDR)
                        : (d.joint_type[j] | (d.joint_enabled[j] ? 16 : 0) | (d.joint_dof_dim[2 * j] << 8) | (d.joint_dof_dim[2 * j + 1] << 12));
@@ -238,13 +266,13 @@ NB2_DEV bool solve_joint(const nb2_model_desc& d, const nb2_control_view& ctl, c
     Xf X_wp = X_pj;
     Xf pose_p = X_pj;
     if (id_p >= 0) {
-        bp = load_body(bodies + id_p * BR_SIZE);
+        bp = load_body(bodies + id_p * bstride, cbodies + id_p * BR_SIZE);
         pose_p = bp.X;
         X_wp = xmul(pose_p, X_wp);
     } else {
         bp.X = pose_p;  // tf_a of the correction helpers is pose_p = X_pj for world-attached joints
     }
-    BodyView bc = load_body(bodies + id_c * BR_SIZE);
+    BodyView bc = load_body(bodies + id_c * bstride, cbodies + id_c * BR_SIZE);
     const Xf pose_c = bc.X;
     const Xf X_wc = xmul(pose_c, X_cj);
     if (bp.inv_m == 0.0f && bc.inv_m == 0.0f) return false;
@@ -252,8 +280,10 @@ NB2_DEV bool solve_joint(const nb2_model_desc& d, const nb2_control_view& ctl, c
     const Xf rel_pose = xmul(xinv(X_wp), X_wc);
     const V3 rel_p = rel_pose.p;
     const V3 x_p = X_wp.p, x_c = X_wc.p;
-    const int axis_start = jc ? jc_int(jc, JC_AXIS) : d.joint_qd_start[j];
-    const int target_start = jc ? jc_int(jc, JC_TARGET) : d.joint_target_q_start[j];
+    // read only by the paths that index the Model with them (distance joints, linear dofs, no joint cache), so that the rows of the
+    // other joints issue no global load for them
+    auto axis_start_of = [&]() { return jc && !tpl ? jc_int(jc, JC_AXIS) : d.joint_qd_start[j]; };
+    auto target_start_of = [&]() { return jc && !tpl ? jc_int(jc, JC_TARGET) : d.joint_target_q_start[j]; };
     const int lin_count = (hdr >> 8) & 15, ang_count = (hdr >> 12) & 15;
     // xpoint(pose, com) of both bodies; the static world's centre of mass is the zero vector
     const V3 wcom_p = id_p >= 0 ? bp.wcom : xpoint(pose_p, V3());
@@ -262,6 +292,7 @@ NB2_DEV bool solve_joint(const nb2_model_desc& d, const nb2_control_view& ctl, c
 
     if (type == JT_DISTANCE) {
         V3 r_p = x_p - wcom_p, r_c = x_c - wcom_c;
+        const int axis_start = axis_start_of();
         float lower = d.joint_limit_lower[axis_start], upper = d.joint_limit_upper[axis_start];
         if (lower < 0.0f && upper < 0.0f) return false;
         V3 ad = x_c - x_p;
@@ -291,7 +322,7 @@ NB2_DEV bool solve_joint(const nb2_model_desc& d, const nb2_control_view& ctl, c
         }
     } else {
         // without linear dofs gather_axes returns AxisSetup() (its axis loop does not run, no division is taken): skip its loads
-        const AxisSetup s = lin_count == 0 ? AxisSetup() : gather_axes(d, ctl, axis_start, target_start, 0, lin_count);
+        const AxisSetup s = lin_count == 0 ? AxisSetup() : gather_axes(d, ctl, axis_start_of(), target_start_of(), 0, lin_count);
         V3 proj = rel_p;
 #pragma unroll
         for (int dim = 0; dim < 3; ++dim) {
@@ -372,7 +403,7 @@ NB2_DEV bool solve_joint(const nb2_model_desc& d, const nb2_control_view& ctl, c
             g1 = qscale(g1, scale);
             g2 = qscale(g2, scale);
         }
-        const AxisSetup s = jc ? load_axis_setup(jc + JC_ANG) : gather_axes(d, ctl, axis_start, target_start, lin_count, ang_count);
+        const AxisSetup s = jc ? load_axis_setup(jc + JC_ANG, jt) : gather_axes(d, ctl, axis_start_of(), target_start_of(), lin_count, ang_count);
         const Q4 qc_inv = qconj(q_c);
         const Q4 hp = qscale(q_p, 0.5f);
         NB2_ROW_UNROLL
@@ -423,7 +454,8 @@ NB2_DEV bool solve_joint(const nb2_model_desc& d, const nb2_control_view& ctl, c
 }
 
 // apply_joint_forces for one joint (kernels.py:945-1075): wrench subtracted from the parent / added to the child.
-NB2_DEV bool joint_force_wrench(const nb2_model_desc& d, const float* joint_f, int j, int body0, const float* bodies, Deltas& out) {
+NB2_DEV bool joint_force_wrench(const nb2_model_desc& d, const float* joint_f, int j, int body0, const float* bodies, int bstride,
+                                const float* cbodies, Deltas& out) {
     const int type = d.joint_type[j];
     if (!d.joint_enabled[j] || type == JT_FIXED || type == JT_ROD) return false;
     const int qd_start = d.joint_qd_start[j];
@@ -449,14 +481,14 @@ NB2_DEV bool joint_force_wrench(const nb2_model_desc& d, const float* joint_f, i
     Xf X_wp = X_pj, pose_p = X_pj;
     V3 com_p;
     if (id_p >= 0) {
-        pose_p = ldx(bodies + id_p * BR_SIZE + BR_Q);
+        pose_p = ldx(bodies + id_p * bstride + BR_Q);
         X_wp = xmul(pose_p, X_wp);
-        com_p = ld3(bodies + id_p * BR_SIZE + BR_COM);
+        com_p = ld3(cbodies + id_p * BR_SIZE + BR_COM);
     }
     V3 r_p = X_wp.p - xpoint(pose_p, com_p);
-    Xf pose_c = ldx(bodies + id_c * BR_SIZE + BR_Q);
+    Xf pose_c = ldx(bodies + id_c * bstride + BR_Q);
     Xf X_wc = xmul(pose_c, X_cj);
-    V3 r_c = X_wc.p - xpoint(pose_c, ld3(bodies + id_c * BR_SIZE + BR_COM));
+    V3 r_c = X_wc.p - xpoint(pose_c, ld3(cbodies + id_c * BR_SIZE + BR_COM));
     if (type == JT_BALL) {
         t_total = V3(joint_f[qd_start], joint_f[qd_start + 1], joint_f[qd_start + 2]);
     } else {
@@ -482,10 +514,10 @@ NB2_DEV void store_deltas(float* rec, const Deltas& dl, float active) {
 }
 
 // apply_body_deltas for one body held in shared memory (kernels.py:864-933), in place.
-NB2_HELPER void apply_delta(float* rec, V3 dlin, V3 dang, float inv_weight, bool weighted, float dt) {
-    const float inv_m = rec[BR_INVM];
+NB2_HELPER void apply_delta(float* rec, const float* crec, V3 dlin, V3 dang, float inv_weight, bool weighted, float dt) {
+    const float inv_m = crec[BR_INVM];
     if (inv_m == 0.0f) return;
-    const M33 inv_I = ldm(rec + BR_INVI), I = ldm(rec + BR_I);
+    const M33 inv_I = ldm(crec + BR_INVI), I = ldm(crec + BR_I);
     const V3 p0 = ld3(rec + BR_Q);
     const Q4 q0(rec[BR_Q + 3], rec[BR_Q + 4], rec[BR_Q + 5], rec[BR_Q + 6]);
     const V3 v0 = ld3(rec + BR_QD), w0 = ld3(rec + BR_QD + 3);
@@ -505,7 +537,7 @@ NB2_HELPER void apply_delta(float* rec, V3 dlin, V3 dang, float inv_weight, bool
     Q4 q1 = qadd(q0, Q4(q0.w * hh.x + hh.y * q0.z - q0.y * hh.z, q0.w * hh.y + hh.z * q0.x - q0.z * hh.x,
                         q0.w * hh.z + hh.x * q0.y - q0.x * hh.y, -hh.x * q0.x - hh.y * q0.y - hh.z * q0.z));
     q1 = qunit(q1);
-    const V3 com = ld3(rec + BR_COM);
+    const V3 com = ld3(crec + BR_COM);
     const V3 x_com = ld3(rec + BR_WCOM);  // p0 + qrot(q0, com)
     const V3 com1 = qrot(q1, com);
     V3 p1 = x_com + dp * dt;
@@ -557,17 +589,21 @@ NB2_GPU void bulk_commit_and_drain() {
 NB2_GPU void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // Shared-memory plan of one CTA (NE environments), in floats.  Identical on host and device.
+// tpl (template mode): one template copy of MB body records and MJ joint cache records for the CTA, first (so that the body
+// constants sit at a fixed address), then per-env body records of BR_DYN words and joint records of JT_SIZE words.
 struct XpbdPlan {
-    int bodies, jcache, cpair, ccache, extra, drec, mbar, total;  // offsets of the per-CTA regions
+    int bodies, tbody, jcache, tjcache, cpair, ccache, extra, drec, mbar, total;  // offsets of the per-CTA regions
     int rec_cap;                                           // delta records per env; the region doubles as the TMA staging area
 };
-__host__ __device__ inline XpbdPlan xpbd_plan(int NE, int MB, int MJ, int CC, bool ex, bool joint_cache, int contact_cache = 0) {
+__host__ __device__ inline XpbdPlan xpbd_plan(int NE, int MB, int MJ, int CC, bool ex, bool joint_cache, int contact_cache, bool tpl) {
     XpbdPlan o;
     auto up4 = [](int x) { return (x + 3) & ~3; };
     o.rec_cap = MB > MJ ? (MB > CC ? MB : CC) : (MJ > CC ? MJ : CC);
-    o.bodies = 0;
-    o.jcache = up4(o.bodies + NE * MB * BR_SIZE);
-    o.cpair = up4(o.jcache + (joint_cache ? NE * MJ * JC_SIZE : 0));
+    o.tbody = 0;
+    o.tjcache = up4(o.tbody + (tpl ? MB * BR_SIZE : 0));
+    o.bodies = up4(o.tjcache + (joint_cache && tpl ? MJ * JC_SIZE : 0));
+    o.jcache = up4(o.bodies + NE * MB * (tpl ? BR_DYN : BR_SIZE));
+    o.cpair = up4(o.jcache + (joint_cache ? NE * MJ * (tpl ? JT_SIZE : JC_SIZE) : 0));
     o.ccache = up4(o.cpair + NE * CC);
     o.extra = up4(o.ccache + NE * contact_cache * CC_SIZE);
     o.drec = up4(o.extra + (ex ? NE * MB * 14 : 0));
@@ -582,21 +618,27 @@ enum { ST_Q = 0, ST_QD = 7, ST_COM = 13, ST_INVM = 16, ST_I = 17, ST_INVI = 26, 
 // position delta, weighted contact impulses for Contacts.force, joint impulses for State.body_parent_f); it is a second
 // instantiation so the plain step pays neither registers nor shared memory for them.
 //
+// TPL = true (template mode, xpbd_template_step_kernel, plain step only): every environment's body and joint constants equal the
+// CTA's first environment's, bit for bit and in environment-relative indices (nb2_model.xpbd_template, detected on the host); the
+// CTA keeps one copy of them and each environment only its state and Control-derived targets.  Each layout is its own kernel: with
+// both bodies behind one branch in a single kernel, the general one ran 5 % slower (box_stacks_xpbd, H100).
+//
 // WARPS warps per CTA, each warp = 32/L environments.  All warps of a CTA walk the same code at about the same time, so the
 // 6 500-instruction iteration body (far larger than the 32 KB L1.5 instruction cache) is fetched once per CTA instead of once per
 // warp; one-warp CTAs each at their own PC stall on instruction fetch.
 #ifndef NB2_XPBD_MIN_WARPS
 #define NB2_XPBD_MIN_WARPS 16  // resident warps per SM the register allocation must allow (16 -> 128 registers)
 #endif
-template <int L, bool EX, int WARPS>
-__global__ void __launch_bounds__(32 * WARPS, (WARPS >= NB2_XPBD_MIN_WARPS ? 1 : NB2_XPBD_MIN_WARPS / WARPS))
-xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_view sout, nb2_control_view ctl, int use_contacts_flags,
-                 float dt, int flags, int contact_cap, int contact_cache) {
+template <int L, bool EX, int WARPS, bool TPL>
+NB2_GPU void xpbd_step_body(const DevModel& M, const nb2_xpbd_params& P, const nb2_state_view& sin, const nb2_state_view& sout,
+                            const nb2_control_view& ctl, int use_contacts_flags, float dt, int flags, int contact_cap, int contact_cache) {
     const int use_contacts = use_contacts_flags & NB2_XPBD_USE_CONTACTS;
     const bool want_cimp = EX && use_contacts && (use_contacts_flags & NB2_XPBD_CONTACT_IMPULSE);
     const bool want_jimp = EX && sout.body_parent_f != nullptr;
     const bool want_init = EX && (P.enable_restitution || P.compute_body_velocity_from_position_delta);
     const bool joint_cache = (flags & XF_JOINT_CACHE) != 0;
+    constexpr bool tpl = TPL;
+    constexpr int bstride = tpl ? int(BR_DYN) : int(BR_SIZE);
     constexpr int G = 32 / L;
     constexpr int NE = G * WARPS;
     extern __shared__ __align__(16) float smem[];
@@ -613,14 +655,17 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
     const int env = env0 + slot;
     const bool live = env < M.env_count;
     const nb2_model_desc& d = M.d;
-    const XpbdPlan plan = xpbd_plan(NE, M.max_env_bodies, M.max_env_joints, contact_cap, EX, joint_cache, contact_cache);
+    const XpbdPlan plan = xpbd_plan(NE, M.max_env_bodies, M.max_env_joints, contact_cap, EX, joint_cache, contact_cache, tpl);
     float* ccache = smem + plan.ccache + slot * contact_cache * CC_SIZE;  // first `contact_cache` contacts of the environment
-    float* bodies = smem + plan.bodies + slot * M.max_env_bodies * BR_SIZE;
+    float* bodies = smem + plan.bodies + slot * M.max_env_bodies * bstride;
+    float* const tbody = smem + plan.tbody;             // template mode: the constants of the CTA's first environment's bodies
+    const float* cbodies = tpl ? tbody : bodies;        // constant part of the body records
     float* drec = smem + plan.drec + slot * plan.rec_cap * DR_SIZE;
     int* cpair = reinterpret_cast<int*>(smem + plan.cpair) + slot * contact_cap;
     float* init_qd = smem + plan.extra + slot * M.max_env_bodies * 14;  // EX only: state_in poses + twists (13/body)
     float* bcnt = init_qd + M.max_env_bodies * 13;                       // EX only: active contacts per body
-    float* jcache = joint_cache ? smem + plan.jcache + slot * M.max_env_joints * JC_SIZE : nullptr;
+    float* jcache = joint_cache ? smem + plan.jcache + slot * M.max_env_joints * (tpl ? JT_SIZE : JC_SIZE) : nullptr;
+    float* const tjcache = smem + plan.tjcache;  // template mode: the joint cache records of the CTA's first environment
     float* stage = smem + plan.drec;  // CTA-wide staging area of the bulk copies (the delta records are not live then)
     unsigned long long* mbar = reinterpret_cast<unsigned long long*>(smem + plan.mbar);
 
@@ -637,7 +682,9 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
     // CTA-uniform decision: the CTA's body run [cb0, cb0 + cnb) must be 16-byte aligned in every array it is copied from / to
     const int env_last = min(env0 + NE, M.env_count);
     const int cb0 = M.env_body_start[env0], cnb = M.env_body_start[env_last] - cb0;
-    bool tma = (flags & XF_TMA) != 0 && cnb > 0 && (cb0 & 3) == 0 && (cnb & 3) == 0 && cnb * ST_PER_BODY <= NE * plan.rec_cap * DR_SIZE;
+    // template mode stages the state only (ST_Q, ST_QD): the constants are gathered once for the template below
+    const int st_words = tpl ? ST_COM : ST_PER_BODY;
+    bool tma = (flags & XF_TMA) != 0 && cnb > 0 && (cb0 & 3) == 0 && (cnb & 3) == 0 && cnb * st_words <= NE * plan.rec_cap * DR_SIZE;
     if (tma) {
         const uintptr_t a = reinterpret_cast<uintptr_t>(sin.body_q) | reinterpret_cast<uintptr_t>(sin.body_qd) |
                             reinterpret_cast<uintptr_t>(sout.body_q) | reinterpret_cast<uintptr_t>(sout.body_qd) |
@@ -649,14 +696,34 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
         if (threadIdx.x == 0) mbar_init(mbar, 1);
         __syncthreads();
         if (threadIdx.x == 0) {
-            mbar_expect_tx(mbar, unsigned(cnb) * ST_PER_BODY * 4u);
+            mbar_expect_tx(mbar, unsigned(cnb) * unsigned(st_words) * 4u);
             bulk_g2s(stage + ST_Q * cnb, sin.body_q + 7 * size_t(cb0), unsigned(cnb) * 28u, mbar);
             bulk_g2s(stage + ST_QD * cnb, sin.body_qd + 6 * size_t(cb0), unsigned(cnb) * 24u, mbar);
-            bulk_g2s(stage + ST_COM * cnb, d.body_com + 3 * size_t(cb0), unsigned(cnb) * 12u, mbar);
-            bulk_g2s(stage + ST_INVM * cnb, d.body_inv_mass + size_t(cb0), unsigned(cnb) * 4u, mbar);
-            bulk_g2s(stage + ST_I * cnb, d.body_inertia + 9 * size_t(cb0), unsigned(cnb) * 36u, mbar);
-            bulk_g2s(stage + ST_INVI * cnb, d.body_inv_inertia + 9 * size_t(cb0), unsigned(cnb) * 36u, mbar);
+            if (!tpl) {
+                bulk_g2s(stage + ST_COM * cnb, d.body_com + 3 * size_t(cb0), unsigned(cnb) * 12u, mbar);
+                bulk_g2s(stage + ST_INVM * cnb, d.body_inv_mass + size_t(cb0), unsigned(cnb) * 4u, mbar);
+                bulk_g2s(stage + ST_I * cnb, d.body_inertia + 9 * size_t(cb0), unsigned(cnb) * 36u, mbar);
+                bulk_g2s(stage + ST_INVI * cnb, d.body_inv_inertia + 9 * size_t(cb0), unsigned(cnb) * 36u, mbar);
+            }
         }
+    }
+    if (tpl) {  // the template: the CTA's first environment's body constants and joint cache records, one thread each
+        const int tnb = M.env_body_start[env0 + 1] - cb0, tj0 = M.env_joint_start[env0], tnj = M.env_joint_start[env0 + 1] - tj0;
+        for (int t = threadIdx.x; t < tnb; t += blockDim.x) {
+            const int gb = cb0 + t;
+            float* rec = tbody + t * BR_SIZE;
+            const bool kin = (d.body_flags[gb] & BODY_KINEMATIC) != 0;
+#pragma unroll
+            for (int k = 0; k < 3; ++k) rec[BR_COM + k] = d.body_com[3 * gb + k];
+            rec[BR_INVM] = kin ? 0.0f : d.body_inv_mass[gb];
+#pragma unroll
+            for (int k = 0; k < 9; ++k) {
+                rec[BR_INVI + k] = kin ? 0.0f : d.body_inv_inertia[9 * gb + k];
+                rec[BR_I + k] = d.body_inertia[9 * gb + k];
+            }
+        }
+        if (joint_cache)
+            for (int t = threadIdx.x; t < tnj; t += blockDim.x) fill_joint_cache(d, ctl, tjcache + t * JC_SIZE, tj0 + t);
     }
     // (while the copies are in flight) contact -> body incidence and the joint cache
     for (int c = l; c < nc; c += L) {
@@ -690,29 +757,32 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
     if (jcache)
         for (int j = l; j < nj; j += L) {
             const int gj = j0 + j;
-            float* jc = jcache + j * JC_SIZE;
-            const int lin_count = d.joint_dof_dim[2 * gj], ang_count = d.joint_dof_dim[2 * gj + 1];
-            const int axis_start = d.joint_qd_start[gj], target_start = d.joint_target_q_start[gj];
-            stx(jc + JC_XP, ldx(d.joint_X_p + 7 * gj));
-            stx(jc + JC_XC, ldx(d.joint_X_c + 7 * gj));
-            store_axis_setup(jc + JC_ANG, gather_axes(d, ctl, axis_start, target_start, lin_count, ang_count));
-            jc[JC_HDR] = __int_as_float(d.joint_type[gj] | (d.joint_enabled[gj] ? 16 : 0) | (lin_count << 8) | (ang_count << 12));
-            jc[JC_CHILD] = __int_as_float(d.joint_child[gj]);
-            jc[JC_PARENT] = __int_as_float(d.joint_parent[gj]);
-            jc[JC_AXIS] = __int_as_float(axis_start);
-            jc[JC_TARGET] = __int_as_float(target_start);
+            if (tpl)  // this environment's Control part of the angular AxisSetup
+                store_axis_targets(jcache + j * JT_SIZE, gather_axes(d, ctl, d.joint_qd_start[gj], d.joint_target_q_start[gj],
+                                                                     d.joint_dof_dim[2 * gj], d.joint_dof_dim[2 * gj + 1]));
+            else
+                fill_joint_cache(d, ctl, jcache + j * JC_SIZE, gj);
         }
     if (tma) mbar_wait(mbar, 0);
     for (int b = l; b < nb; b += L) {
         const int gb = b0 + b;
-        float* rec = bodies + b * BR_SIZE;
-        const bool kin = (d.body_flags[gb] & BODY_KINEMATIC) != 0;  // _update_effective_inv_mass_inertia (solver.py:173-187)
+        float* rec = bodies + b * bstride;
         if (tma) {
             const int sb = gb - cb0;
 #pragma unroll
             for (int k = 0; k < 7; ++k) rec[BR_Q + k] = stage[ST_Q * cnb + 7 * sb + k];
 #pragma unroll
             for (int k = 0; k < 6; ++k) rec[BR_QD + k] = stage[ST_QD * cnb + 6 * sb + k];
+        } else {
+#pragma unroll
+            for (int k = 0; k < 7; ++k) rec[BR_Q + k] = sin.body_q[7 * gb + k];
+#pragma unroll
+            for (int k = 0; k < 6; ++k) rec[BR_QD + k] = sin.body_qd[6 * gb + k];
+        }
+        if (tpl) continue;
+        const bool kin = (d.body_flags[gb] & BODY_KINEMATIC) != 0;  // _update_effective_inv_mass_inertia (solver.py:173-187)
+        if (tma) {
+            const int sb = gb - cb0;
 #pragma unroll
             for (int k = 0; k < 3; ++k) rec[BR_COM + k] = stage[ST_COM * cnb + 3 * sb + k];
             rec[BR_INVM] = kin ? 0.0f : stage[ST_INVM * cnb + sb];
@@ -722,10 +792,6 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
                 rec[BR_I + k] = stage[ST_I * cnb + 9 * sb + k];
             }
         } else {
-#pragma unroll
-            for (int k = 0; k < 7; ++k) rec[BR_Q + k] = sin.body_q[7 * gb + k];
-#pragma unroll
-            for (int k = 0; k < 6; ++k) rec[BR_QD + k] = sin.body_qd[6 * gb + k];
 #pragma unroll
             for (int k = 0; k < 3; ++k) rec[BR_COM + k] = d.body_com[3 * gb + k];
             rec[BR_INVM] = kin ? 0.0f : d.body_inv_mass[gb];
@@ -739,8 +805,9 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
     if (want_init)
         for (int b = l; b < nb; b += L)
 #pragma unroll
-            for (int k = 0; k < 13; ++k) init_qd[b * 13 + k] = bodies[b * BR_SIZE + BR_Q + k];  // q (7) then qd (6) are adjacent
-    if (tma) __syncthreads();  // every warp has unpacked its bodies: the staging area becomes the delta records
+            for (int k = 0; k < 13; ++k) init_qd[b * 13 + k] = bodies[b * bstride + BR_Q + k];  // q (7) then qd (6) are adjacent
+    // every warp has unpacked its bodies: the staging area becomes the delta records; the template is complete
+    if (tma || tpl) __syncthreads();
     else __syncwarp();
     // ---- contact -> body incidence as two bit masks per body lane (contact c touches this body on side A / side B) --------------
     // Contact order is the summation order; a mask walk visits exactly the incident records in that order instead of rescanning
@@ -758,7 +825,7 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
     // ---- apply_joint_forces: per-joint wrenches, then ordered per-body accumulation into a body_f copy ----
     for (int j = l; j < nj; j += L) {
         Deltas w;
-        bool act = joint_force_wrench(d, ctl.joint_f, j0 + j, b0, bodies, w);
+        bool act = joint_force_wrench(d, ctl.joint_f, j0 + j, b0, bodies, bstride, cbodies, w);
         if (!act) w = Deltas();
         store_deltas(drec + j * DR_SIZE, w, act ? 1.0f : 0.0f);
         if (want_jimp) {  // child-side wrench * dt opens the joint's impulse accumulator (kernels.py:1018-1019, 1074-1075)
@@ -772,7 +839,8 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
     // ---- integrate_bodies (solver.py:64-107) ----------------------------------------------------
     for (int b = l; b < nb; b += L) {
         const int gb = b0 + b;
-        float* rec = bodies + b * BR_SIZE;
+        float* rec = bodies + b * bstride;
+        const float* crec = cbodies + b * BR_SIZE;
         V3 f0 = ld3(sin.body_f + 6 * gb), t0 = ld3(sin.body_f + 6 * gb + 3);
         for (int k = M.body_joint_start[gb]; k < M.body_joint_start[gb + 1]; ++k) {
             const int e = M.body_joint_entry[k];
@@ -783,16 +851,16 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
             }
         }
         if ((d.body_flags[gb] & BODY_KINEMATIC) != 0) {  // kinematic bodies pass through (solver.py:132-139)
-            st3(rec + BR_WCOM, xpoint(ldx(rec + BR_Q), ld3(rec + BR_COM)));
+            st3(rec + BR_WCOM, xpoint(ldx(rec + BR_Q), ld3(crec + BR_COM)));
             continue;
         }
         const V3 x0 = ld3(rec + BR_Q);
         const Q4 r0(rec[BR_Q + 3], rec[BR_Q + 4], rec[BR_Q + 5], rec[BR_Q + 6]);
         const V3 v0 = ld3(rec + BR_QD), w0 = ld3(rec + BR_QD + 3);
-        const V3 com = ld3(rec + BR_COM);
-        const float inv_mass = rec[BR_INVM];  // not kinematic here: the effective value is the model's
-        const M33 inertia = ldm(rec + BR_I);
-        const M33 inv_inertia = ldm(rec + BR_INVI);
+        const V3 com = ld3(crec + BR_COM);
+        const float inv_mass = crec[BR_INVM];  // not kinematic here: the effective value is the model's
+        const M33 inertia = ldm(crec + BR_I);
+        const M33 inv_inertia = ldm(crec + BR_INVI);
         int wi = d.body_world[gb];
         if (wi < 0) wi += d.gravity_count;
         const V3 g = ld3(d.gravity + 3 * wi);
@@ -835,8 +903,8 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
                     // A side never consumed by a body (static world) and not reported: its arithmetic is skipped.  Identity
                     // transform and zero centre of mass reduce xpoint(X, p) to (+0) + p and r to the contact point itself.
                     const bool need_a = ba >= 0 || want_cimp, need_b = bb >= 0 || want_cimp;
-                    BodyView A = ba >= 0 ? load_body(bodies + ba * BR_SIZE) : static_body();
-                    BodyView B = bb >= 0 ? load_body(bodies + bb * BR_SIZE) : static_body();
+                    BodyView A = ba >= 0 ? load_body(bodies + ba * bstride, cbodies + ba * BR_SIZE) : static_body();
+                    BodyView B = bb >= 0 ? load_body(bodies + bb * bstride, cbodies + bb * BR_SIZE) : static_body();
                     const bool cached = c < contact_cache;
                     const float* cc = ccache + c * CC_SIZE;
                     const V3 p0 = cached ? ld3(cc + CC_P0) : V3(cb[CF_P0X * T + s], cb[CF_P0Y * T + s], cb[CF_P0Z * T + s]);
@@ -953,7 +1021,7 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
                         if (bb == b) { dlin += ld3(r + 6); dang += ld3(r + 9); cnt += 1.0f; }
                     }
                 }
-                apply_delta(bodies + b * BR_SIZE, dlin, dang, cnt, P.rigid_contact_con_weighting != 0, dt);
+                apply_delta(bodies + b * bstride, cbodies + b * BR_SIZE, dlin, dang, cnt, P.rigid_contact_con_weighting != 0, dt);
                 if (want_cimp) bcnt[b] = cnt;
             }
             __syncwarp();
@@ -986,7 +1054,9 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
             // ---- [iteration] solve_body_joints (kernels.py:1513-2044) + ordered per-body apply
             for (int j = l; j < nj; j += L) {
                 Deltas dl;
-                bool act = solve_joint(d, ctl, P, j0 + j, b0, bodies, jcache ? jcache + j * JC_SIZE : nullptr, dt, lin_alpha_dt,
+                const float* jc = !jcache ? nullptr : (tpl ? tjcache : jcache) + j * JC_SIZE;
+                const float* jt = !jcache ? nullptr : (tpl ? jcache + j * JT_SIZE : jcache + j * JC_SIZE + JC_TGT);
+                bool act = solve_joint(d, ctl, P, j0 + j, tpl && jcache ? cb0 : b0, bodies, bstride, cbodies, jc, jt, tpl, dt, lin_alpha_dt,
                                        ang_alpha_dt, dl);
                 if (!act) dl = Deltas();
                 store_deltas(drec + j * DR_SIZE, dl, act ? 1.0f : 0.0f);
@@ -1009,7 +1079,7 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
                     if (e & 1) { dlin += ld3(r + 6); dang += ld3(r + 9); }
                     else { dlin += ld3(r + 0); dang += ld3(r + 3); }
                 }
-                apply_delta(bodies + b * BR_SIZE, dlin, dang, 0.0f, false, dt);
+                apply_delta(bodies + b * bstride, cbodies + b * BR_SIZE, dlin, dang, 0.0f, false, dt);
             }
             __syncwarp();
         }
@@ -1041,9 +1111,9 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
         if (P.compute_body_velocity_from_position_delta) {
             for (int b = l; b < nb; b += L) {
                 if ((d.body_flags[b0 + b] & BODY_KINEMATIC) != 0) continue;
-                float* rec = bodies + b * BR_SIZE;
+                float* rec = bodies + b * bstride;
                 const Xf pose = ldx(rec + BR_Q), prev = ldx(init_qd + b * 13);
-                const V3 com = ld3(rec + BR_COM);
+                const V3 com = ld3(cbodies + b * BR_SIZE + BR_COM);
                 const V3 x_com = pose.p + qrot(pose.q, com), x_prev = prev.p + qrot(prev.q, com);
                 const V3 v = (x_com - x_prev) / dt;
                 const Q4 dq = qmul(pose.q, qconj(prev.q));
@@ -1069,10 +1139,12 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
                     if (sa >= 0) restitution += d.shape_material_restitution[sa], ++mat_nonzero;
                     if (sb >= 0) restitution += d.shape_material_restitution[sb], ++mat_nonzero;
                     restitution /= float(mat_nonzero);
-                    const float* ra_rec = ba >= 0 ? bodies + ba * BR_SIZE : nullptr;
-                    const float* rb_rec = bb >= 0 ? bodies + bb * BR_SIZE : nullptr;
+                    const float* ra_rec = ba >= 0 ? bodies + ba * bstride : nullptr;
+                    const float* rb_rec = bb >= 0 ? bodies + bb * bstride : nullptr;
+                    const float* ra_c = ba >= 0 ? cbodies + ba * BR_SIZE : nullptr;
+                    const float* rb_c = bb >= 0 ? cbodies + bb * BR_SIZE : nullptr;
                     const Xf Xa = ba >= 0 ? ldx(init_qd + ba * 13) : Xf(), Xb = bb >= 0 ? ldx(init_qd + bb * 13) : Xf();
-                    const V3 com_a = ba >= 0 ? ld3(ra_rec + BR_COM) : V3(), com_b = bb >= 0 ? ld3(rb_rec + BR_COM) : V3();
+                    const V3 com_a = ba >= 0 ? ld3(ra_c + BR_COM) : V3(), com_b = bb >= 0 ? ld3(rb_c + BR_COM) : V3();
                     const V3 p0(cb[CF_P0X * T + s], cb[CF_P0Y * T + s], cb[CF_P0Z * T + s]);
                     const V3 p1(cb[CF_P1X * T + s], cb[CF_P1Y * T + s], cb[CF_P1Z * T + s]);
                     const V3 o0(cb[CF_O0X * T + s], cb[CF_O0Y * T + s], cb[CF_O0Z * T + s]);
@@ -1087,8 +1159,8 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
                         if (ba >= 0) {
                             int wi = d.body_world[b0 + ba];
                             if (wi < 0) wi += d.gravity_count;
-                            m_inv_a = ra_rec[BR_INVM];
-                            I_inv_a = ldm(ra_rec + BR_INVI);
+                            m_inv_a = ra_c[BR_INVM];
+                            I_inv_a = ldm(ra_c + BR_INVI);
                             v_a = (cross(ld3(init_qd + ba * 13 + 10), r_a) + ld3(init_qd + ba * 13 + 7)) + ld3(d.gravity + 3 * wi) * dt;
                             v_a_new = cross(ld3(ra_rec + BR_QD + 3), r_a) + ld3(ra_rec + BR_QD);
                             rxn_a = qrot_inv(Xa.q, cross(r_a, n));
@@ -1097,8 +1169,8 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
                         if (bb >= 0) {
                             int wi = d.body_world[b0 + bb];
                             if (wi < 0) wi += d.gravity_count;
-                            m_inv_b = rb_rec[BR_INVM];
-                            I_inv_b = ldm(rb_rec + BR_INVI);
+                            m_inv_b = rb_c[BR_INVM];
+                            I_inv_b = ldm(rb_c + BR_INVI);
                             v_b = (cross(ld3(init_qd + bb * 13 + 10), r_b) + ld3(init_qd + bb * 13 + 7)) + ld3(d.gravity + 3 * wi) * dt;
                             v_b_new = cross(ld3(rb_rec + BR_QD + 3), r_b) + ld3(rb_rec + BR_QD);
                             rxn_b = qrot_inv(Xb.q, cross(r_b, n));
@@ -1135,7 +1207,7 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
                     if (ba == b) { dlin += ld3(r + 0); dang += ld3(r + 3); }
                     if (bb == b) { dlin += ld3(r + 6); dang += ld3(r + 9); }
                 }
-                float* rec = bodies + b * BR_SIZE;
+                float* rec = bodies + b * bstride;
                 st3(rec + BR_QD, ld3(rec + BR_QD) + dlin);
                 st3(rec + BR_QD + 3, ld3(rec + BR_QD + 3) + dang);
             }
@@ -1148,7 +1220,7 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
         __syncthreads();  // all warps are done with their delta records: the region is the staging area again
         for (int b = l; b < nb; b += L) {
             const int sb = b0 + b - cb0;
-            const float* rec = bodies + b * BR_SIZE;
+            const float* rec = bodies + b * bstride;
 #pragma unroll
             for (int k = 0; k < 7; ++k) stage[ST_Q * cnb + 7 * sb + k] = rec[BR_Q + k];
 #pragma unroll
@@ -1166,13 +1238,26 @@ xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_vi
     }
     for (int b = l; b < nb; b += L) {
         const int gb = b0 + b;
-        const float* rec = bodies + b * BR_SIZE;
+        const float* rec = bodies + b * bstride;
 #pragma unroll
         for (int k = 0; k < 7; ++k) sout.body_q[7 * gb + k] = rec[BR_Q + k];
 #pragma unroll
         for (int k = 0; k < 6; ++k) sout.body_qd[6 * gb + k] = rec[BR_QD + k];
     }
     NB2_PHASE_CLOCK(PC_END);
+}
+
+template <int L, bool EX, int WARPS>
+__global__ void __launch_bounds__(32 * WARPS, (WARPS >= NB2_XPBD_MIN_WARPS ? 1 : NB2_XPBD_MIN_WARPS / WARPS))
+xpbd_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_view sout, nb2_control_view ctl, int use_contacts_flags,
+                 float dt, int flags, int contact_cap, int contact_cache) {
+    xpbd_step_body<L, EX, WARPS, false>(M, P, sin, sout, ctl, use_contacts_flags, dt, flags, contact_cap, contact_cache);
+}
+template <int L, int WARPS>
+__global__ void __launch_bounds__(32 * WARPS, (WARPS >= NB2_XPBD_MIN_WARPS ? 1 : NB2_XPBD_MIN_WARPS / WARPS))
+xpbd_template_step_kernel(DevModel M, nb2_xpbd_params P, nb2_state_view sin, nb2_state_view sout, nb2_control_view ctl,
+                          int use_contacts_flags, float dt, int flags, int contact_cap, int contact_cache) {
+    xpbd_step_body<L, false, WARPS, true>(M, P, sin, sout, ctl, use_contacts_flags, dt, flags, contact_cap, contact_cache);
 }
 
 // SolverXPBD.update_contacts (solver_xpbd.py:864-925): force[i] = weighted impulse of exported contact i / dt
@@ -1243,48 +1328,80 @@ static nb2_status launch_xpbd_W(nb2_model* m, const nb2_xpbd_params& p, const nb
         return NB2_ERR_CAPACITY;
     }
     // Budget: the CTAs of one SM share 227 KB (+1 KB reserved each); the batch wants >= ceil(envs / (G * 132)) resident warps per SM to
-    // stay a single wave on an H100 SXM.  The per-joint cache rides along when it does not cost that residency.
+    // stay a single wave on an H100 SXM.  The per-joint cache rides along when it does not cost that residency; the contact-constant
+    // cache takes as many contacts per env as still fit (up to the contact bound).
     static const bool cache_enabled = std::getenv("NB2_XPBD_NO_JOINT_CACHE") == nullptr;  // A/B switch
     static const int tma_enabled = env_int("NB2_XPBD_TMA", 1), phase_sync = env_int("NB2_XPBD_PHASE_SYNC", 1);
-    int flags = (tma_enabled ? XF_TMA : 0) | (phase_sync >= 1 ? XF_PHASE_SYNC : 0) | (phase_sync >= 2 ? XF_PHASE_SYNC_FINE : 0);
-    XpbdPlan plan = xpbd_plan(NE, M.max_env_bodies, M.max_env_joints, contact_cap, EX, false);
-    if (cache_enabled && M.d.joint_count > 0) {
-        const XpbdPlan with_cache = xpbd_plan(NE, M.max_env_bodies, M.max_env_joints, contact_cap, EX, true);
-        const int want_ctas = (16 + WARPS - 1) / WARPS;  // 16 warps per SM keep 4096 two-env warps in one wave on 132 SMs
-        if ((size_t(with_cache.total) * sizeof(float) + 1024) * want_ctas <= 227 * 1024 || size_t(plan.total) * sizeof(float) * want_ctas > 227 * 1024) {
-            if (size_t(with_cache.total) * sizeof(float) <= 220 * 1024) {
-                plan = with_cache;
-                flags |= XF_JOINT_CACHE;
+    static const int cc_enabled = env_int("NB2_XPBD_CONTACT_CACHE", 1);
+    const int want_ctas = (16 + WARPS - 1) / WARPS;  // 16 warps per SM keep 4096 two-env warps in one wave on 132 SMs
+    struct Choice {
+        XpbdPlan plan;
+        int base_total;  // plan words before the contact-constant cache
+        bool joint_cache;
+        int contact_cache;
+    };
+    auto choose = [&](bool tpl) {
+        Choice c;
+        c.joint_cache = false;
+        c.plan = xpbd_plan(NE, M.max_env_bodies, M.max_env_joints, contact_cap, EX, false, 0, tpl);
+        if (cache_enabled && M.d.joint_count > 0) {
+            const XpbdPlan with_cache = xpbd_plan(NE, M.max_env_bodies, M.max_env_joints, contact_cap, EX, true, 0, tpl);
+            if ((size_t(with_cache.total) * sizeof(float) + 1024) * want_ctas <= 227 * 1024 ||
+                size_t(c.plan.total) * sizeof(float) * want_ctas > 227 * 1024) {
+                if (size_t(with_cache.total) * sizeof(float) <= 220 * 1024) {
+                    c.plan = with_cache;
+                    c.joint_cache = true;
+                }
             }
         }
-    }
-    // contact-constant cache: as many contacts per env as still fit (up to the contact bound), keeping the residency above
-    int contact_cache = 0;
-    {
-        static const int cc_enabled = env_int("NB2_XPBD_CONTACT_CACHE", 1);
-        const int want_ctas = (16 + WARPS - 1) / WARPS;
+        c.base_total = c.plan.total;
+        c.contact_cache = 0;
         const size_t budget = (size_t(227) * 1024) / want_ctas - 1024 - 64;
-        const size_t base = size_t(plan.total) * sizeof(float);
+        const size_t base = size_t(c.plan.total) * sizeof(float);
         if (cc_enabled && use_contacts && base < budget) {
-            contact_cache = int(std::min<size_t>((budget - base) / (size_t(NE) * CC_SIZE * sizeof(float)), size_t(contact_cap)));
-            if (contact_cache > 0)
-                plan = xpbd_plan(NE, M.max_env_bodies, M.max_env_joints, contact_cap, EX, (flags & XF_JOINT_CACHE) != 0, contact_cache);
+            c.contact_cache = int(std::min<size_t>((budget - base) / (size_t(NE) * CC_SIZE * sizeof(float)), size_t(contact_cap)));
+            if (c.contact_cache > 0)
+                c.plan = xpbd_plan(NE, M.max_env_bodies, M.max_env_joints, contact_cap, EX, c.joint_cache, c.contact_cache, tpl);
+        }
+        return c;
+    };
+    // Template mode (every environment's constants equal, nb2_model.xpbd_template; plain step only): the constant parts of the
+    // body records and of the joint cache are held once per CTA, which pays for itself only with several environments per CTA.
+    // It is taken when the general layout leaves contacts uncached and the template layout, with the same choice of joint cache,
+    // is no larger; the freed bytes then go to the contact-constant cache.
+    Choice pick = choose(false);
+    bool tpl = false;
+    if (!EX && m->xpbd_template && pick.contact_cache < contact_cap) {
+        const Choice t = choose(true);
+        if (t.joint_cache == pick.joint_cache && t.base_total <= pick.base_total) {
+            pick = t;
+            tpl = true;
         }
     }
+    const XpbdPlan plan = pick.plan;
+    const int contact_cache = pick.contact_cache;
+    const int flags = (tma_enabled ? XF_TMA : 0) | (phase_sync >= 1 ? XF_PHASE_SYNC : 0) | (phase_sync >= 2 ? XF_PHASE_SYNC_FINE : 0) |
+                      (pick.joint_cache ? XF_JOINT_CACHE : 0);
     const size_t smem = size_t(plan.total) * sizeof(float);
     if (smem > 220 * 1024 + 6 * 1024) {
         set_error("xpbd_step: environment too large for the fused shared-memory kernel (bodies/contacts per env)");
         return NB2_ERR_CAPACITY;
     }
-    if (smem > 48 * 1024)
-        NB2_CUDA_CHECK(cudaFuncSetAttribute(xpbd_step_kernel<L, EX, WARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+    auto kernel = xpbd_step_kernel<L, EX, WARPS>;
+    if constexpr (!EX)
+        if (tpl) kernel = xpbd_template_step_kernel<L, WARPS>;
+    if (smem > 48 * 1024) NB2_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
     // ask for the largest shared-memory carve-out so that 16 warps' worth of CTAs fit per SM
     static const int carveout = std::getenv("NB2_XPBD_CARVEOUT") ? std::atoi(std::getenv("NB2_XPBD_CARVEOUT")) : int(cudaSharedmemCarveoutMaxShared);
-    NB2_CUDA_CHECK(cudaFuncSetAttribute(xpbd_step_kernel<L, EX, WARPS>, cudaFuncAttributePreferredSharedMemoryCarveout, carveout));
+    NB2_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, carveout));
     // A/B switch: pad the grid with idle CTAs up to this many (does a grid below the SM count change the issue rate?)
     static const int min_grid = env_int("NB2_XPBD_MIN_GRID", 0);
     const int grid = blocks < min_grid ? min_grid : blocks;
-    xpbd_step_kernel<L, EX, WARPS><<<grid, 32 * WARPS, smem, s>>>(M, p, in, out, ctl, use_contacts, dt, flags, contact_cap, contact_cache);
+    m->xpbd_last_plan[0] = tpl ? 1 : 0;
+    m->xpbd_last_plan[1] = contact_cache;
+    m->xpbd_last_plan[2] = contact_cap;
+    m->xpbd_last_plan[3] = int(smem);
+    kernel<<<grid, 32 * WARPS, smem, s>>>(M, p, in, out, ctl, use_contacts, dt, flags, contact_cap, contact_cache);
     count_launch();
     NB2_CUDA_CHECK(cudaGetLastError());
     return NB2_OK;
@@ -1309,7 +1426,7 @@ static nb2_status launch_xpbd_L(nb2_model* m, const nb2_xpbd_params& p, const nb
     auto fits = [&](int w) {
         const int ne = (32 / L) * w;
         const int cap = m->contacts_imported ? m->dev.max_env_contact_slots : std::min(m->dev.max_env_contact_slots, m->max_env_contacts);
-        return size_t(xpbd_plan(ne, m->dev.max_env_bodies, m->dev.max_env_joints, cap, EX, false).total) * sizeof(float) <= 200 * 1024;
+        return size_t(xpbd_plan(ne, m->dev.max_env_bodies, m->dev.max_env_joints, cap, EX, false, 0, false).total) * sizeof(float) <= 200 * 1024;
     };
     if (warps >= 16 && !fits(16)) warps = 4;
     if (warps >= 4 && warps < 16 && !fits(4)) warps = 1;
